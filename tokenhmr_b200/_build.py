@@ -1,4 +1,5 @@
-"""Builds libtokenhmr_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
+"""Builds libtokenhmr_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU), and next to the test suite
+the kernel probe tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers)."""
 from __future__ import annotations
 
 import hashlib
@@ -11,6 +12,9 @@ PKG_DIR = Path(__file__).resolve().parent
 CSRC = PKG_DIR / "csrc"
 LIB_PATH = PKG_DIR / "libtokenhmr_b200.so"
 STAMP = PKG_DIR / ".libtokenhmr_b200.stamp"
+PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "kernel_probe.cu"
+PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_probe.so"
+PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_probe.stamp"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -18,6 +22,10 @@ NVCC_FLAGS = [
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-shared",
 ]
+# The probe is loaded into the same process as the library and compiles the same inline functions, whose static locals
+# (e.g. the "kernel attributes configured" flags of the launchers) would otherwise be merged with the library's by the
+# dynamic linker.  Hidden visibility keeps every one of them private to the probe; its wrappers are exported explicitly.
+PROBE_FLAGS = ["-Xcompiler", "-fvisibility=hidden"]
 
 
 def _nvcc() -> str:
@@ -27,22 +35,22 @@ def _nvcc() -> str:
     return "nvcc"
 
 
-def source_hash() -> str:
+def source_hash(probe: bool = False) -> str:
     h = hashlib.sha256()
     files = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + sorted((PKG_DIR.parent / "include").glob("*.h"))
+    if probe:
+        files += sorted(PROBE_SRC.parent.glob("*.cu"))
     for f in files:
         h.update(f.name.encode())
         h.update(f.read_bytes())
-    h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(" ".join(NVCC_FLAGS + (PROBE_FLAGS if probe else [])).encode())
     return h.hexdigest()
 
 
-def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile csrc/tokenhmr_b200.cu -> libtokenhmr_b200.so (no-op when sources are unchanged)."""
-    want = source_hash()
-    if not force and LIB_PATH.exists() and STAMP.exists() and STAMP.read_text().strip() == want:
-        return LIB_PATH
-    cmd = [_nvcc(), *NVCC_FLAGS, "-o", str(LIB_PATH), str(CSRC / "tokenhmr_b200.cu")]  # cudart linked statically (nvcc default)
+def _compile(src: Path, out: Path, stamp: Path, flags: list, want: str, force: bool, verbose: bool) -> Path:
+    if not force and out.exists() and stamp.exists() and stamp.read_text().strip() == want:
+        return out
+    cmd = [_nvcc(), *flags, "-o", str(out), str(src)]  # cudart linked statically (nvcc default)
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
         print(" ".join(cmd), file=sys.stderr)
@@ -51,8 +59,22 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         raise RuntimeError(f"nvcc failed ({res.returncode}):\n{res.stdout}\n{res.stderr}")
     if verbose:
         print(res.stderr, file=sys.stderr)
-    STAMP.write_text(want)
-    return LIB_PATH
+    stamp.write_text(want)
+    return out
+
+
+def build_probe(force: bool = False, verbose: bool = False) -> Path:
+    """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so (no-op when sources are unchanged)."""
+    return _compile(PROBE_SRC, PROBE_PATH, PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, source_hash(probe=True), force, verbose)
+
+
+def build(force: bool = False, verbose: bool = False) -> Path:
+    """Compile csrc/tokenhmr_b200.cu -> libtokenhmr_b200.so, and the kernel probe when the test sources are present
+    (no-op when sources are unchanged)."""
+    path = _compile(CSRC / "tokenhmr_b200.cu", LIB_PATH, STAMP, NVCC_FLAGS, source_hash(), force, verbose)
+    if PROBE_SRC.exists():
+        build_probe(force, verbose)
+    return path
 
 
 if __name__ == "__main__":
