@@ -37,12 +37,18 @@ struct GemmDesc {
 };
 
 // Tile width: wide tiles move fewer operand bytes per MAC (every k-block moves (128 + BN) * 128 bytes for
-// 128 * BN * 64 MACs), so they win unless they leave SMs idle.  Cost model per k-block in cycles on an H100 SM:
-// max(MMA at 2048 fp16 MAC/clk, operand feed at ~32 B/clk from L2), plus a fixed per-k-block overhead.
-inline int pick_bn(int M, int N, int force) {
+// 128 * BN * 64 MACs), so they win unless they leave SMs idle or their epilogue dominates.  Cost model per tile in
+// cycles on an H100 SM: per k-block max(MMA at 2048 fp16 MAC/clk, operand feed at ~32 B/clk from L2) plus a fixed
+// overhead, plus the epilogue.  The epilogue terms are fitted to the ViT GEMMs (M = 12288) on an H100 80GB HBM3 at a
+// 400 W power limit, so that the model picks the measured-faster width at all five of them: ~28 us per 128 x 256
+// tile (eight 32-column staging chunks) against ~3.5 us per 128 x 128 tile (two 64-column chunks), so 256 wins only
+// at long K (fc2, K = 5120); the narrower tiles are scaled from 128.  The row arg-min epilogue (VQ) is not staged and
+// is not charged.
+inline int pick_bn(int M, int N, int K, bool staged_epilogue, int force) {
   if (force) return force;
   const int sms = num_sms();
   const int tm = (M + kGemmBM - 1) / kGemmBM;
+  const int num_kb = (K + kGemmBK - 1) / kGemmBK;
   int best = 256;
   double best_cost = -1;
   const int cands[4] = {256, 128, 64, 32};
@@ -52,7 +58,8 @@ inline int pick_bn(int M, int N, int force) {
     const long waves = (tiles + sms - 1) / sms;
     const double mma = 4.0 * bn;
     const double feed = (128.0 + bn) * 128.0 / 32.0;
-    const double cost = waves * ((mma > feed ? mma : feed) + 40.0);
+    const double epilogue = !staged_epilogue ? 0.0 : bn == 256 ? 55000.0 : 7000.0 * bn / 128;
+    const double cost = waves * (num_kb * ((mma > feed ? mma : feed) + 40.0) + epilogue);
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = bn; }
   }
   return best;
@@ -63,7 +70,7 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   THMR_CHECK(d.out32 || d.out16 || d.argmin_out, "gemm: no output");
   const int cluster = d.force_bn == 512 ? 2 : 1;
   THMR_CHECK(cluster == 1 || !d.argmin_out, "gemm: block_n 512 (CTA pair) does not support the arg-min modes");
-  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.force_bn);
+  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.K, d.argmin_out == nullptr, d.force_bn);
   THMR_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: bad block_n %d", bn);
   GemmParams& p = plan->p;
   memset(&p, 0, sizeof(p));

@@ -15,9 +15,10 @@
 // once the consumers of BOTH CTAs have released it (the empty barrier counts the consumer warps of the cluster).
 //
 // The producer runs ahead into the next tile while the consumers store the current one, so the epilogue overlaps the
-// operand loads of the next tile.  The epilogue works straight from the accumulator registers and handles every
-// option: alpha scale, bias, a residual (may alias out32: same element, same thread), residual tables, padded-sequence
-// masking, activations, fp32 and / or fp16 outputs, and the row-argmin modes of the VQ nearest-code search.
+// operand loads of the next tile.  The element-wise epilogue stages the accumulators through shared memory and stores
+// whole row segments (gemm_epilogue_rows); it handles alpha scale, bias, a residual (may alias out32: same element,
+// same thread), residual tables, padded-sequence masking, activations, fp32 and / or fp16 outputs.  The row-argmin
+// modes of the VQ nearest-code search work straight from the accumulator registers.
 //
 // The same kernel runs the implicit-GEMM Conv1d (k=3, dilated) of the pose-token decoder: k-blocks are
 // grouped in "taps", each tap reads the A rows shifted by a row offset (TMA zero-fills out-of-range rows).
@@ -104,13 +105,21 @@ constexpr int kGemmConsumerWarps = 8;
 constexpr int kGemmThreads = 32 * kGemmConsumerWarps + 128;  // two consumer warpgroups + the producer warpgroup
 constexpr int kWarpTma = kGemmConsumerWarps;
 
+// Columns of one epilogue chunk: each consumer warpgroup stages 64 rows x gemm_chunk fp32 accumulators in shared
+// memory.  At BN = 256 the accumulators still held for the later chunks leave registers for the residuals of 32
+// columns only (64 spill); narrower tiles take 64.
+template <int BN>
+constexpr int gemm_chunk() { return BN == 64 || BN == 128 ? 64 : 32; }
+
 template <int BN, int STAGES>
 struct GemmSmem {
   static constexpr uint32_t kABytes = kGemmBM * kGemmBK * 2;
   static constexpr uint32_t kBBytes = BN * kGemmBK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;   // multiple of 1024: every operand tile stays swizzle-aligned
   static constexpr uint32_t kBarOffset = STAGES * kStageBytes;
-  static constexpr uint32_t kTotal = kBarOffset + 256 + 1024;  // barriers, alignment slack
+  static constexpr uint32_t kEpiOffset = kBarOffset + 256;     // epilogue staging, one 64 x chunk block per warpgroup
+  static constexpr uint32_t kEpiBytes = 2 * 64 * gemm_chunk<BN>() * 4;
+  static constexpr uint32_t kTotal = kEpiOffset + kEpiBytes + 1024;  // alignment slack
 };
 
 // Exact-erf GELU (nn.GELU default, vit.py:73).  The epilogue evaluates 63 M of these per MLP layer, so erf uses
@@ -139,53 +148,155 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da
   else wgmma_m64n256k16(acc, da, db, scale_d);
 }
 
-// Epilogue of one accumulator pair (columns col, col + 1 of one row); v1 is ignored when col + 1 >= N.
-__device__ __forceinline__ void gemm_store_pair(const GemmParams& p, int row, int col, float v0, float v1,
-                                                bool vec32, bool vec16) {
-  const bool two = col + 1 < p.N;
-  v0 *= p.alpha;
-  v1 *= p.alpha;
-  if (p.bias) {
-    v0 += __ldg(p.bias + col);
-    if (two) v1 += __ldg(p.bias + col + 1);
-  }
-  if (p.resid) {
-    const float* r = p.resid + static_cast<size_t>(p.resid_mod > 0 ? row % p.resid_mod : row) * p.ldr + col;
-    if (two && vec32) {
-      const float2 r2 = *reinterpret_cast<const float2*>(r);
-      v0 += r2.x; v1 += r2.y;
-    } else {
-      v0 += r[0];
-      if (two) v1 += r[1];
+__device__ __forceinline__ float gemm_act(int act, float v) {
+  return act == kActGelu ? gelu_erf(v) : act == kActRelu ? fmaxf(v, 0.f) : v;
+}
+
+__device__ __forceinline__ bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+// Element-wise epilogue of one consumer warpgroup: its 64 rows x BN columns of accumulators, rows m0w.. of the output.
+// The accumulator fragment (two rows x two columns per 8-column group and thread) goes to a shared-memory chunk of
+// 64 x CH fp32; the warpgroup then walks the chunk row-major, each thread owning 8 consecutive columns ("octets") of
+// two rows, so that every global access is a 16-byte vector of one row (scalar when base, pitch or N forbid it).  All
+// residual loads of a chunk are issued before any of its stores: one memory round trip per chunk instead of one per
+// accumulator pair.  A residual aliasing out32 is safe: each element is read and written by the same thread.
+// Staging layout: row r of the chunk holds CH / 4 16-byte units; unit u sits at u ^ swz(r) (low three bits), which keeps
+// both the fragment writes (four rows x 32 bytes per half-warp) and the row reads (eight rows of one unit per
+// quarter-warp) free of bank conflicts.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
+                                                   int m0w, int n0, int M_eff, uint32_t bar_id, bool vec_r, bool vec32,
+                                                   bool vec16) {
+  constexpr int CH = gemm_chunk<BN>();
+  constexpr int OCT = CH / 8;          // octets per chunk row
+  constexpr int ITEMS = OCT / 2;       // (row, octet) items per thread and chunk: 64 * OCT / 128
+  const int lane = threadIdx.x & 31;
+  const int w4 = (threadIdx.x >> 5) & 3;
+  // fragment side: rows (16 w4 + lane / 4 + 8 i), columns 8 j + 2 (lane % 4) + {0, 1}
+  const int fr = w4 * 16 + (lane >> 2);
+  const int fswz = (((lane >> 2) & 3) << 1) | ((lane >> 4) & 1);   // swz(fr), fr % 8 = lane / 4
+  // row side: item k is row (8 (w4 + 4 (k % 2)) + lane % 8), octet (4 (k / 2) + lane / 8) of the chunk
+  const int rswz = ((lane & 3) << 1) | ((lane >> 2) & 1);          // swz(row), row % 8 = lane % 8
+  // row terms, once per tile: the thread's two rows, whether they exist, the padded-sequence mask, the residual row
+  int rows[2];
+  bool live[2], keep[2];
+  const float* rres[2];
+#pragma unroll
+  for (int ri = 0; ri < 2; ++ri) {
+    const int row = m0w + 8 * (w4 + 4 * ri) + (lane & 7);
+    rows[ri] = row;
+    live[ri] = row < M_eff;
+    keep[ri] = true;
+    if (p.seq_pitch > 0) {
+      const int rr = row % p.seq_pitch;
+      keep[ri] = rr >= p.seq_lo && rr < p.seq_hi;
     }
+    // a masked row is stored as zero whatever its residual, so the residual is not read
+    rres[ri] = (p.resid && live[ri] && keep[ri])
+                   ? p.resid + static_cast<size_t>(p.resid_mod > 0 ? row % p.resid_mod : row) * p.ldr
+                   : nullptr;
   }
-  if (p.seq_pitch > 0) {
-    const int rr = row % p.seq_pitch;
-    if (rr < p.seq_lo || rr >= p.seq_hi) { v0 = 0.f; v1 = 0.f; }
-  }
-  if (p.act32) {
-    if (p.act == kActGelu) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-    else if (p.act == kActRelu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-  }
-  if (p.out32) {
-    float* o = p.out32 + static_cast<size_t>(row) * p.ld32 + col;
-    if (two && vec32) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-    else {
-      o[0] = v0;
-      if (two) o[1] = v1;
+
+#pragma unroll
+  for (int c = 0; c < BN / CH; ++c) {
+#pragma unroll
+    for (int j = 0; j < OCT; ++j) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int u = 2 * j + ((lane & 3) >> 1);
+        const int a = 4 * (c * OCT + j) + 2 * i;
+        sts_f32x2(stage + 4 * ((fr + 8 * i) * CH + (((u & ~7) | ((u ^ fswz) & 7)) << 2) + 2 * (lane & 1)), acc[a],
+                  acc[a + 1]);
+      }
     }
-  }
-  if (p.out16) {
-    if (!p.act32) {
-      if (p.act == kActGelu) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-      else if (p.act == kActRelu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+    named_barrier_sync(bar_id, 128);
+
+    const int ccol = n0 + c * CH + 8 * (lane >> 3);   // first column of octet 0 of this thread in the chunk
+    float bias[ITEMS / 2][8];
+    float res[ITEMS][8];
+#pragma unroll
+    for (int ob = 0; ob < ITEMS / 2; ++ob)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int col = ccol + 32 * ob + e;
+        bias[ob][e] = (p.bias && col < p.N) ? __ldg(p.bias + col) : 0.f;
+      }
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const int col = ccol + 32 * (k >> 1);
+      const float* r = rres[k & 1];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) res[k][e] = 0.f;
+      if (r != nullptr && col < p.N) {
+        if (vec_r && col + 8 <= p.N) {
+          const float4 x0 = *reinterpret_cast<const float4*>(r + col);
+          const float4 x1 = *reinterpret_cast<const float4*>(r + col + 4);
+          res[k][0] = x0.x; res[k][1] = x0.y; res[k][2] = x0.z; res[k][3] = x0.w;
+          res[k][4] = x1.x; res[k][5] = x1.y; res[k][6] = x1.z; res[k][7] = x1.w;
+        } else {
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (col + e < p.N) res[k][e] = r[col + e];
+        }
+      }
     }
-    __half* o = p.out16 + static_cast<size_t>(row) * p.ld16 + col;
-    if (two && vec16) *reinterpret_cast<__half2*>(o) = __floats2half2_rn(v0, v1);
-    else {
-      o[0] = __float2half_rn(v0);
-      if (two) o[1] = __float2half_rn(v1);
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const int ri = k & 1;
+      const int lr = 8 * (w4 + 4 * ri) + (lane & 7);
+      const int oct = 4 * (k >> 1) + (lane >> 3);
+      const int col = ccol + 32 * (k >> 1);
+      const int row = rows[ri];
+      if (!live[ri] || col >= p.N) continue;
+      float v[8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int u = 2 * oct + h;
+        const float4 s = lds_f32x4(stage + 4 * (lr * CH + (((u & ~7) | ((u ^ rswz) & 7)) << 2)));
+        v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
+      }
+      // alpha * acc + bias + resid, mask, activation: the operation order of the reference epilogue, element for element
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[e] *= p.alpha;
+        if (p.bias) v[e] += bias[k >> 1][e];
+        if (p.resid) v[e] += res[k][e];
+        if (!keep[ri]) v[e] = 0.f;
+        if (p.act32) v[e] = gemm_act(p.act, v[e]);
+      }
+      const bool full = col + 8 <= p.N;
+      if (p.out32) {
+        float* o = p.out32 + static_cast<size_t>(row) * p.ld32 + col;
+        if (full && vec32) {
+          reinterpret_cast<float4*>(o)[0] = make_float4(v[0], v[1], v[2], v[3]);
+          reinterpret_cast<float4*>(o)[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (col + e < p.N) o[e] = v[e];
+        }
+      }
+      if (p.out16) {
+        if (!p.act32) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = gemm_act(p.act, v[e]);
+        }
+        __half* o = p.out16 + static_cast<size_t>(row) * p.ld16 + col;
+        if (full && vec16) {
+          uint4 q;
+          __half2* h2 = reinterpret_cast<__half2*>(&q);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) h2[e] = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
+          *reinterpret_cast<uint4*>(o) = q;
+        } else {
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (col + e < p.N) o[e] = __float2half_rn(v[e]);
+        }
+      }
     }
+    // the next chunk (or tile) overwrites the staging block
+    named_barrier_sync(bar_id, 128);
   }
 }
 
@@ -269,8 +380,11 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int wg = warp >> 2;
   const uint32_t smem_base = smem_u32(smem);
-  const bool vec32 = (!p.out32 || p.ld32 % 2 == 0) && (!p.resid || p.ldr % 2 == 0);
-  const bool vec16 = p.out16 && p.ld16 % 2 == 0;
+  // 16-byte vectors of one row: the base and the pitch keep every 8-column group 16-byte aligned
+  const bool vec_r = p.resid && p.ldr % 4 == 0 && aligned16(p.resid);
+  const bool vec32 = p.out32 && p.ld32 % 4 == 0 && aligned16(p.out32);
+  const bool vec16 = p.out16 && p.ld16 % 8 == 0 && aligned16(p.out16);
+  const uint32_t epi_stage = smem_base + S::kEpiOffset + wg * 64 * gemm_chunk<BN>() * 4;
   const bool screen = p.argmin_out != nullptr && p.screen_rows != nullptr;
   const float m2a = -2.0f * p.alpha;
   // accumulator fragment of this thread: rows r0, r0 + 8 of the tile, columns 8 j + c0 + {0, 1}
@@ -383,18 +497,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     } else {
-      // ---- element-wise epilogue straight from the accumulators
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = m0 + r0 + 8 * i;
-        if (row < M_eff) {
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int col = n0 + 8 * j + c0;
-            if (col < p.N) gemm_store_pair(p, row, col, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], vec32, vec16);
-          }
-        }
-      }
+      gemm_epilogue_rows<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16);
     }
   }
   // the peer may still arrive on this CTA's barriers: neither CTA leaves before both are done

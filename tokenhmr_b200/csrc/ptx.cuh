@@ -19,6 +19,21 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// shared-memory accesses by 32-bit shared address (the compiler cannot tell a pointer into the aligned dynamic
+// smem block from a global one and would emit generic accesses); ordered against named_barrier_sync
+__device__ __forceinline__ void sts_f32x2(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y));
+}
+__device__ __forceinline__ float4 lds_f32x4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
+}
+// barrier `id` (1..15; 0 is __syncthreads) over `threads` threads, e.g. one warpgroup
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 __device__ __forceinline__ uint32_t lane_id() {
   uint32_t l;
   asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
