@@ -18,7 +18,7 @@
  *
  * Numeric contract (DESIGN.md): every Linear / Conv / attention product rounds its two operands to f16 and
  * accumulates in fp32 on the tensor cores (wgmma); LayerNorm, softmax, GELU, residual streams, 6D->rotation,
- * SMPL skinning and projection are fp32.
+ * SMPL skinning and projection are fp32.  thmr_config::strict and thmr_config::fp8 select the two other modes.
  */
 #ifndef TOKENHMR_B200_H_
 #define TOKENHMR_B200_H_
@@ -236,6 +236,13 @@ typedef struct thmr_config {
                    * (another forward of this engine's weights replayed on a second stream, TokenHMRPipeline(streams=2)):
                    * no kernel of this library waits for another CTA of its grid, so both values select the same
                    * schedules; the field is kept so that callers can state the intent. */
+  int fp8;      /* 0: as `strict` says.  1: the ViT's QKV, fc1 (+ GELU) and fc2 GEMMs run on block-scaled e4m3 operands
+                 * (DeepSeek-V3's fine-grained scheme, DESIGN.md §2): activations carry one power-of-two scale per (row,
+                 * 128 columns), weights one per 128 x 128 block; each 128-wide k-block accumulates on the FP8 tensor
+                 * cores and is promoted into fp32 with its two scales.  Everything else is as in the default mode.
+                 * qkv_w, fc1_w and fc2_w of every thmr_vit_block then point to e4m3 [out, in] codes and
+                 * thmr_weights::block_scales_host gives their scales (packed by tokenhmr_b200/weights.py with fp8=True).
+                 * Not with strict (THMR_ERR_INVALID). */
 } thmr_config;
 
 /* Weight pointers, packed by the host loader (tokenhmr_b200/weights.py) from the reference state_dicts.
@@ -248,6 +255,12 @@ typedef struct thmr_vit_block {
   const void* fc1_w; const float* fc1_b;      /* [4D,D] */
   const void* fc2_w; const float* fc2_b;      /* [D,4D] */
 } thmr_vit_block;
+
+/* FP8 mode: fp32 power-of-two scales of one ViT block's e4m3 weights, [ceil(out / 128), in / 128] row-major, one per
+ * 128 x 128 block of the [out, in] matrix (the weight is the code times its block's scale). */
+typedef struct thmr_vit_block_scales {
+  const float *qkv_ws, *fc1_ws, *fc2_ws;
+} thmr_vit_block_scales;
 
 typedef struct thmr_dec_layer {
   const float *ln0_g, *ln0_b;
@@ -295,6 +308,8 @@ typedef struct thmr_weights {
   thmr_conv conv_up[8];                        /* after each Upsample */
   thmr_conv res_conv1[8], res_conv2[8];        /* Resnet1D blocks in stored order (dilation rate^(depth-1) ... 1) */
   thmr_conv conv_post, conv_out;               /* W -> W, W -> 6 */
+  /* FP8 mode (thmr_config::fp8): host array [vit_depth] of the e4m3 weight scales; ignored (may be NULL) otherwise */
+  const thmr_vit_block_scales* block_scales_host;
 } thmr_weights;
 
 typedef struct thmr_outputs {                  /* all fp32, caller-allocated; any pointer may be NULL */

@@ -34,12 +34,16 @@ class Config(Structure):
                 ("cls_token_inter", c_int), ("cls_blocks", c_int),
                 ("code_dim", c_int), ("tok_width", c_int), ("tok_depth", c_int), ("tok_dilation_rate", c_int),
                 ("tok_joints", c_int), ("n_upsample", c_int), ("upsample_sizes", c_int * 8),
-                ("focal_length", c_float), ("strict", c_int), ("concurrent", c_int)]
+                ("focal_length", c_float), ("strict", c_int), ("concurrent", c_int), ("fp8", c_int)]
 
 
 class VitBlock(Structure):
     _fields_ = [(n, c_void_p) for n in ("ln1_g", "ln1_b", "qkv_w", "qkv_b", "proj_w", "proj_b", "ln2_g", "ln2_b",
                                         "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
+
+
+class VitBlockScales(Structure):
+    _fields_ = [(n, c_void_p) for n in ("qkv_ws", "fc1_ws", "fc2_ws")]
 
 
 class DecLayer(Structure):
@@ -68,7 +72,8 @@ class Weights(Structure):
                 ("mn_w", c_void_p), ("mn_b", c_void_p), ("mn_ln_g", c_void_p), ("mn_ln_b", c_void_p),
                 ("cls_w", c_void_p), ("cls_b", c_void_p),
                 ("codebook_t", c_void_p), ("conv_in", Conv), ("conv_up", Conv * 8),
-                ("res_conv1", Conv * 8), ("res_conv2", Conv * 8), ("conv_post", Conv), ("conv_out", Conv)]
+                ("res_conv1", Conv * 8), ("res_conv2", Conv * 8), ("conv_post", Conv), ("conv_out", Conv),
+                ("block_scales_host", POINTER(VitBlockScales))]
 
 
 class TokConv(Structure):

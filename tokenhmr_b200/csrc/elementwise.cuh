@@ -261,6 +261,84 @@ inline int layernorm_launch(const float* x, const float* gamma, const float* bet
 }
 
 // ------------------------------------------------------------------------------------------------
+// LayerNorm with an e4m3 output: the FP8 A operand of the ViT's QKV and fc1 GEMMs.  Same two-pass fp32 statistics and
+// output expression as layernorm_reg_kernel; C = 128 * VEC4, so the lane's float4 i of the row lies in 128-column group
+// i.  Per (row, group): s = the smallest power of two with amax / s <= 448, codes = cvt.rn.satfinite(y / s), scales to
+// ys[group * lds + row] (the k-block-major layout of GemmParams::a_scale).  y32 (nullable) receives the fp32 values
+// before quantisation.
+template <int VEC4>
+__global__ void __launch_bounds__(256)
+layernorm_e4m3_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                      uint8_t* __restrict__ y8, float* __restrict__ ys, int lds, float* __restrict__ y32, int R,
+                      float eps, unsigned long long* stamp) {
+  constexpr int C = VEC4 * 128;
+  stamp_start(stamp);
+  extern __shared__ float4 s_gb[];   // [2][C/4]
+  float4* sg = s_gb;
+  float4* sb = s_gb + C / 4;
+  for (int c = threadIdx.x; c < C / 4; c += blockDim.x) {
+    sg[c] = reinterpret_cast<const float4*>(gamma)[c];
+    sb[c] = reinterpret_cast<const float4*>(beta)[c];
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int warps_total = (gridDim.x * blockDim.x) >> 5;
+  for (int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; warp < R; warp += warps_total) {
+    const float* xr = x + static_cast<size_t>(warp) * C;
+    float4 v[VEC4];
+#pragma unroll
+    for (int i = 0; i < VEC4; ++i) v[i] = *reinterpret_cast<const float4*>(xr + (i * 32 + lane) * 4);
+    float s_lo = 0.f, s_hi = 0.f;
+#pragma unroll
+    for (int i = 0; i < VEC4; ++i) {
+      s_lo += v[i].x; s_hi += v[i].y;
+      s_lo += v[i].z; s_hi += v[i].w;
+    }
+    const float mean = warp_sum(s_lo + s_hi) / C;
+    float q_lo = 0.f, q_hi = 0.f;
+#pragma unroll
+    for (int i = 0; i < VEC4; ++i) {
+      const float d0 = v[i].x - mean, d1 = v[i].y - mean, d2 = v[i].z - mean, d3 = v[i].w - mean;
+      q_lo = fmaf(d0, d0, q_lo); q_hi = fmaf(d1, d1, q_hi);
+      q_lo = fmaf(d2, d2, q_lo); q_hi = fmaf(d3, d3, q_hi);
+    }
+    const float rstd = rsqrtf(warp_sum(q_lo + q_hi) / C + eps);
+#pragma unroll
+    for (int i = 0; i < VEC4; ++i) {
+      const int c = (i * 32 + lane) * 4;
+      const float4 g = sg[c >> 2];
+      const float4 bb = sb[c >> 2];
+      float4 o;
+      o.x = fmaf((v[i].x - mean) * rstd, g.x, bb.x);
+      o.y = fmaf((v[i].y - mean) * rstd, g.y, bb.y);
+      o.z = fmaf((v[i].z - mean) * rstd, g.z, bb.z);
+      o.w = fmaf((v[i].w - mean) * rstd, g.w, bb.w);
+      if (y32) *reinterpret_cast<float4*>(y32 + static_cast<size_t>(warp) * C + c) = o;
+      const float s = e4m3_scale(warp_max(fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w)))));
+      const float inv = 1.0f / s;
+      const uint32_t q = cvt_e4m3x2(o.x * inv, o.y * inv) | (static_cast<uint32_t>(cvt_e4m3x2(o.z * inv, o.w * inv)) << 16);
+      *reinterpret_cast<uint32_t*>(y8 + static_cast<size_t>(warp) * C + c) = q;
+      if (lane == 0) ys[static_cast<size_t>(i) * lds + warp] = s;
+    }
+  }
+}
+
+inline int layernorm_e4m3_launch(const float* x, const float* gamma, const float* beta, uint8_t* y8, float* ys, int lds,
+                                 float* y32, int R, int C, float eps, cudaStream_t st,
+                                 unsigned long long* stamp = nullptr) {
+  THMR_CHECK(C == 1280 || C == 1024 || C == 128, "layernorm e4m3: C=%d (128, 1024 or 1280)", C);
+  THMR_CHECK(lds >= R, "layernorm e4m3: scale pitch %d < rows %d", lds, R);
+  int grid = (R + 7) / 8;
+  if (grid > num_sms() * 4) grid = num_sms() * 4;
+  const size_t smem = 2 * static_cast<size_t>(C) * sizeof(float);
+  if (C == 1280) layernorm_e4m3_kernel<10><<<grid, 256, smem, st>>>(x, gamma, beta, y8, ys, lds, y32, R, eps, stamp);
+  else if (C == 1024) layernorm_e4m3_kernel<8><<<grid, 256, smem, st>>>(x, gamma, beta, y8, ys, lds, y32, R, eps, stamp);
+  else layernorm_e4m3_kernel<1><<<grid, 256, smem, st>>>(x, gamma, beta, y8, ys, lds, y32, R, eps, stamp);
+  THMR_CUDA(cudaGetLastError());
+  return THMR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Row softmax over C = 32*4*VEC4 classes (token_classifier.py:104): logits fp32 -> probs fp32 (the
 // cls_logits_softmax output) + an fp16 copy laid out for the soft-codebook GEMM (quantize_cnn.py:92-93),
 // whose rows live in zero-padded sequences: row r = b*T + t  ->  p16 row b*pitch + lo + t.

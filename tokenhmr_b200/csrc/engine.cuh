@@ -117,6 +117,7 @@ struct thmr_engine {
   thmr_config cfg;
   thmr_weights w;
   std::vector<thmr_vit_block> blocks;
+  std::vector<thmr_vit_block_scales> block_scales;   // fp8 mode only
   std::vector<thmr_dec_layer> dec;
   std::vector<thmr_mixer_block> mixer;
   const thmr_smpl* smpl = nullptr;
@@ -197,6 +198,11 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   float* verts_fb = bp.take<float>(static_cast<size_t>(B) * e->smpl->m.V * 3);
   SmplWs sws;
   smpl_carve(bp, e->smpl->m, B, &sws);
+  // fp8 mode: xn and h hold e4m3 codes inside their fp16 buffers; their power-of-two scales are k-block-major
+  // [cols / 128][ld_sc], ld_sc = M + 128 so that every 128-row tile of every sub-batch reads a full 512-byte run
+  const int ld_sc = M + 128;
+  float* xn_sc = c.fp8 ? bp.take<float>(static_cast<size_t>(D / 128) * ld_sc) : nullptr;
+  float* h_sc = c.fp8 ? bp.take<float>(static_cast<size_t>(c.vit_mlp_ratio * D / 128) * ld_sc) : nullptr;
   const size_t total = (bp.off + 1023) & ~size_t(1023);
   if (!build) return total;
 
@@ -231,6 +237,29 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
     d.bias = bias; d.act = act; d.resid = resid; d.ldr = N;
     d.out32 = o32; d.ld32 = N; d.out16 = o16; d.ld16 = N;
     add_gemm(d);
+  };
+  // fp8 mode: A and B are e4m3 codes with their block scales; o8 (nullable) = e4m3 output + its scales
+  auto linear8 = [&](const uint8_t* A, const float* a_sc, int rows, const void* Wt, const float* w_sc, int N, int K,
+                     const float* bias, int act, float* o32, __half* o16, const float* resid, uint8_t* o8,
+                     float* o8_sc) {
+    GemmDesc d;
+    d.fp8 = 1;
+    d.A = reinterpret_cast<const __half*>(A); d.lda = K; d.a_rows = rows;
+    d.B = static_cast<const __half*>(Wt); d.ldb = K;
+    d.M = rows; d.N = N; d.K = K;
+    d.bias = bias; d.act = act; d.resid = resid; d.ldr = N;
+    d.out32 = o32; d.ld32 = N; d.out16 = o16; d.ld16 = N;
+    d.a_scale = a_sc; d.ld_as = ld_sc; d.w_scale = w_sc;
+    d.out8 = o8; d.ld8 = N; d.out8_scale = o8_sc; d.ld8s = ld_sc;
+    add_gemm(d);
+  };
+  auto ln8 = [&](const float* in, const float* g, const float* b, uint8_t* o8, float* o_sc, int R, int C, float eps) {
+    S.flops = 0;
+    S.bytes = static_cast<double>(R) * C * 5;
+    unsigned long long* sp = slot();
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
+      return layernorm_e4m3_launch(in, g, b, o8, o_sc, ld_sc, nullptr, R, C, eps, st, sp);
+    });
   };
   auto ln = [&](const float* in, const float* g, const float* b, __half* o16, float* o32, int R, int C, float eps,
                 int relu, int out_t) {
@@ -278,7 +307,38 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   __half* qkvs = qkv + r0 * 3 * D;
   __half* aos = ao + r0 * D;
   __half* hs = hbuf + r0 * c.vit_mlp_ratio * D;
-  for (int i = 0; i < c.vit_depth; ++i) {
+  for (int i = 0; i < c.vit_depth && c.fp8; ++i) {
+    // fp8 mode: LN -> e4m3 xn -> QKV (fp16 qkv), attention and proj as by default, LN -> e4m3 xn -> fc1 + GELU ->
+    // e4m3 h -> fc2 into the fp32 residual stream
+    const thmr_vit_block& bw = e->blocks[i];
+    const thmr_vit_block_scales& bs = e->block_scales[i];
+    uint8_t* xn8 = reinterpret_cast<uint8_t*>(xns);
+    uint8_t* h8 = reinterpret_cast<uint8_t*>(hs);
+    const int F = c.vit_mlp_ratio * D;
+    S.tag("vit.layernorm");
+    ln8(xs, bw.ln1_g, bw.ln1_b, xn8, xn_sc + r0, Ms, D, c.vit_ln_eps);
+    S.tag("vit.qkv_gemm");
+    linear8(xn8, xn_sc + r0, Ms, bw.qkv_w, bs.qkv_ws, 3 * D, D, bw.qkv_b, kActNone, nullptr, qkvs, nullptr, nullptr,
+            nullptr);
+    {
+      S.tag("vit.attention", 4.0 * bn * H * 192.0 * 192.0 * 80.0, 4.0 * Ms * D * 2);
+      AttnPlan ap;
+      const int s = attention_make_plan(qkvs, 3 * D, bn, H, aos, D, nullptr, &ap);
+      if (s != THMR_OK) err = s;
+      ap.p.stamp = slot();
+      S.push_back([ap](const RunCtx&, cudaStream_t st) -> int { return attention_dispatch(ap, st); });
+    }
+    S.tag("vit.proj_gemm");
+    linear(aos, D, Ms, bw.proj_w, D, D, bw.proj_b, kActNone, xs, nullptr, xs);
+    S.tag("vit.layernorm");
+    ln8(xs, bw.ln2_g, bw.ln2_b, xn8, xn_sc + r0, Ms, D, c.vit_ln_eps);
+    S.tag("vit.fc1_gelu_gemm");
+    linear8(xn8, xn_sc + r0, Ms, bw.fc1_w, bs.fc1_ws, F, D, bw.fc1_b, kActGelu, nullptr, nullptr, nullptr, h8,
+            h_sc + r0);
+    S.tag("vit.fc2_gemm");
+    linear8(h8, h_sc + r0, Ms, bw.fc2_w, bs.fc2_ws, D, F, bw.fc2_b, kActNone, xs, nullptr, xs, nullptr, nullptr);
+  }
+  for (int i = 0; i < c.vit_depth && !c.fp8; ++i) {
     const thmr_vit_block& bw = e->blocks[i];
     S.tag("vit.layernorm");
     ln(xs, bw.ln1_g, bw.ln1_b, xns, nullptr, Ms, D, c.vit_ln_eps, 0, 0);

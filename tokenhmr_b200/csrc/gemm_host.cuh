@@ -12,6 +12,7 @@ struct GemmPlan {
   int bn;
   int grid;
   int cluster;   // 2: CTA pairs sharing the B tile (gemm_wgmma.cuh)
+  int fp8;       // e4m3 operands (gemm_make_plan_fp8)
 };
 
 struct GemmDesc {
@@ -34,6 +35,12 @@ struct GemmDesc {
   const int* row_map = nullptr; const int* m_dev = nullptr; int m_dev_off = 0;
   int force_bn = 0;   // 32 / 64 / 128 / 256, or 512 = a CTA pair (2-CTA cluster) on a 256 x 256 tile
   unsigned long long* stamp = nullptr;   // in-graph start stamp slot (nullable)
+  // FP8 (GemmParams): A and B point to e4m3 bytes (lda / ldb in elements = bytes), K a multiple of 128; block_n 64 or
+  // 128, 128 with out8.  a_scale [K / 128][ld_as] must hold the tile-padded rows (ld_as >= M rounded up to 128).
+  int fp8 = 0;
+  const float* a_scale = nullptr; int ld_as = 0;
+  const float* w_scale = nullptr;
+  uint8_t* out8 = nullptr; int ld8 = 0; float* out8_scale = nullptr; int ld8s = 0;
 };
 
 // Tile width: wide tiles move fewer operand bytes per MAC (every k-block moves (128 + BN) * 128 bytes for
@@ -65,7 +72,73 @@ inline int pick_bn(int M, int N, int K, bool staged_epilogue, int force) {
   return best;
 }
 
+// FP8 tile width, the same model at FP8 rates: a 128-element k-block moves the bytes of an fp16 64-element one and
+// takes the same MMA time (4096 e4m3 MAC/clk), so per K there are half the k-blocks; each k-block adds the promotion
+// (BN / 2 FMAs per consumer thread, ~BN cycles per SM).  Two accumulator sets leave 64 and 128 only.
+inline int pick_bn_fp8(int M, int N, int K) {
+  const int sms = num_sms();
+  const int tm = (M + kGemmBM - 1) / kGemmBM;
+  const int num_kb = (K + 127) / 128;
+  int best = 128;
+  double best_cost = -1;
+  const int cands[2] = {128, 64};
+  for (int i = 0; i < 2; ++i) {
+    const int bn = cands[i];
+    const long tiles = static_cast<long>(tm) * ((N + bn - 1) / bn);
+    const long waves = (tiles + sms - 1) / sms;
+    const double mma = 4.0 * bn;
+    const double feed = (128.0 + bn) * 128.0 / 32.0;
+    const double cost = waves * (num_kb * ((mma > feed ? mma : feed) + bn + 40.0) + 7000.0 * bn / 128);
+    if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = bn; }
+  }
+  return best;
+}
+
+inline int make_tmap_2d_e4m3(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                             uint32_t box_rows, uint32_t box_cols) {
+  return make_tmap_2d(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, base, rows, cols, ld, box_rows, box_cols,
+                      CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+inline int gemm_make_plan_fp8(const GemmDesc& d, GemmPlan* plan) {
+  THMR_CHECK(d.M > 0 && d.N > 0 && d.K > 0 && d.K % 128 == 0, "gemm fp8: bad shape %dx%dx%d (K %% 128 != 0)", d.M, d.N,
+             d.K);
+  THMR_CHECK(d.out32 || d.out16 || d.out8, "gemm fp8: no output");
+  THMR_CHECK(d.a_scale && d.w_scale, "gemm fp8: missing block scales");
+  THMR_CHECK(!d.argmin_out && d.taps == 1 && !d.m_dev && !d.row_map, "gemm fp8: plain GEMMs only");
+  const long m_pad = (d.M + kGemmBM - 1) / kGemmBM * kGemmBM;
+  THMR_CHECK(d.ld_as >= m_pad && d.ld_as % 4 == 0 && (reinterpret_cast<uintptr_t>(d.a_scale) & 15) == 0,
+             "gemm fp8: activation scales need a 16-byte aligned [K/128][>= %ld] layout (ld_as %d)", m_pad, d.ld_as);
+  int bn = d.force_bn ? d.force_bn : d.out8 ? 128 : pick_bn_fp8(d.M, d.N, d.K);
+  THMR_CHECK(bn == 64 || bn == 128, "gemm fp8: block_n %d (64 or 128)", bn);
+  THMR_CHECK(!d.out8 || (bn == 128 && d.out8_scale && d.ld8s >= d.M && !d.resid && !d.act32 && !d.seq_pitch),
+             "gemm fp8: e4m3 output needs block_n 128, its scale array and no residual / mask / act32");
+  GemmParams& p = plan->p;
+  memset(&p, 0, sizeof(p));
+  p.M = d.M; p.N = d.N; p.K = d.K;
+  p.out32 = d.out32; p.ld32 = d.ld32; p.out16 = d.out16; p.ld16 = d.ld16;
+  p.bias = d.bias; p.resid = d.resid; p.ldr = d.ldr; p.resid_mod = d.resid_mod; p.act = d.act; p.act32 = d.act32;
+  p.seq_pitch = d.seq_pitch; p.seq_lo = d.seq_lo; p.seq_hi = d.seq_hi;
+  p.alpha = d.alpha;
+  p.stamp = d.stamp;
+  p.kblocks_per_tap = d.K / 128;
+  p.a_scale = d.a_scale; p.ld_as = d.ld_as; p.w_scale = d.w_scale;
+  p.out8 = d.out8; p.ld8 = d.ld8; p.out8_scale = d.out8_scale; p.ld8s = d.ld8s;
+  THMR_TRY(make_tmap_2d_e4m3(&plan->tmA, d.A, d.a_rows, d.K, d.lda, kGemmBM, 128));
+  THMR_TRY(make_tmap_2d_e4m3(&plan->tmB, d.B, d.N, d.K, d.ldb, bn, 128));
+  plan->bn = bn;
+  plan->cluster = 1;
+  plan->fp8 = 1;
+  const long tiles_m = (d.M + kGemmBM - 1) / kGemmBM;
+  const long tiles = tiles_m * ((d.N + bn - 1) / bn);
+  p.m_fast = (tiles_m > 1 && d.M < d.N) ? 1 : 0;
+  const long slots = num_sms();
+  plan->grid = static_cast<int>(tiles < slots ? tiles : slots);
+  return THMR_OK;
+}
+
 inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
+  if (d.fp8) return gemm_make_plan_fp8(d, plan);
   THMR_CHECK(d.M > 0 && d.N > 0 && d.K > 0, "gemm: bad shape %dx%dx%d", d.M, d.N, d.K);
   THMR_CHECK(d.out32 || d.out16 || d.argmin_out, "gemm: no output");
   const int cluster = d.force_bn == 512 ? 2 : 1;
@@ -100,6 +173,7 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   THMR_TRY(make_tmap_2d_f16(&plan->tmB, d.B, d.N, d.K, d.ldb, bn / cluster, kGemmBK, CU_TENSOR_MAP_SWIZZLE_128B));
   plan->bn = bn;
   plan->cluster = cluster;
+  plan->fp8 = 0;
   const long tiles_m = (d.M + kGemmBM * cluster - 1) / (kGemmBM * cluster);
   const long tiles = d.argmin_out ? tiles_m : tiles_m * ((d.N + bn - 1) / bn);
   // the CTAs of a wave should share tiles of the larger operand (TileIter)
@@ -109,13 +183,13 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   return THMR_OK;
 }
 
-template <int BN, int STAGES, int CLUSTER = 1>
+template <int BN, int STAGES, int CLUSTER = 1, bool FP8 = false>
 inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
-  using S = GemmSmem<BN, STAGES>;
+  using S = GemmSmem<BN, STAGES, FP8>;
   static_assert(S::kTotal <= 232448, "GEMM shared memory exceeds 227 KB");
   static bool configured = false;
   if (!configured) {
-    THMR_CUDA(cudaFuncSetAttribute(gemm_f16_tn_kernel<BN, STAGES, CLUSTER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    THMR_CUDA(cudaFuncSetAttribute(gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    S::kTotal));
     configured = true;
   }
@@ -131,11 +205,17 @@ inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER>, plan.tmA, plan.tmB, plan.p));
+  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8>, plan.tmA, plan.tmB, plan.p));
   return THMR_OK;
 }
 
 inline int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+  if (plan.fp8) {
+    // the stage ring also carries 512 bytes of activation scales per stage, and the epilogue the row scales
+    if (plan.bn == 128) return gemm_launch_t<128, 5, 1, true>(plan, stream);
+    if (plan.bn == 64) return gemm_launch_t<64, 7, 1, true>(plan, stream);
+    return fail(THMR_ERR_INVALID, "gemm fp8: unsupported block_n %d", plan.bn);
+  }
   if (plan.cluster == 2) return gemm_launch_t<256, 4, 2>(plan, stream);
   switch (plan.bn) {
     case 256: return gemm_launch_t<256, 4>(plan, stream);

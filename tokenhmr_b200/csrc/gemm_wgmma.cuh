@@ -69,6 +69,18 @@ struct GemmParams {
   int m_dev_off;
   unsigned long long* stamp;   // in-graph start stamp (common.cuh stamp_start), nullable
   int m_fast;     // row tile fastest in the tile order (see TileIter)
+  // FP8 operands (gemm_f16_tn_kernel<..., FP8 = true>): A and B are e4m3 with power-of-two block scales, a k-block is
+  // 128 elements.  Each k-block's products accumulate in a fresh register tile that is then promoted into the fp32
+  // accumulator:  acc += tile * (a_scale[kb][row] * w_scale[n / 128][kb]).
+  const float* a_scale;  // [K / 128][ld_as] per (row, k-block), k-block-major: one 512-byte run per 128-row tile
+  int ld_as;             // >= the tile-padded row count, a multiple of 4
+  const float* w_scale;  // [ceil(N / 128)][K / 128] per 128 x 128 block of B
+  // e4m3 output (FP8 only, block_n 128): act(alpha * acc + bias) as codes of one power-of-two scale per (row, 128
+  // columns), i.e. per tile row; the scales go to out8_scale[n / 128][row], the layout a_scale expects
+  uint8_t* out8;   // nullable
+  int ld8;
+  float* out8_scale;
+  int ld8s;
 };
 
 // Tile order shared by the producer and the consumers.  Normal mode: tiles round-robin over CTAs, column tile
@@ -111,15 +123,24 @@ constexpr int kWarpTma = kGemmConsumerWarps;
 template <int BN>
 constexpr int gemm_chunk() { return BN == 64 || BN == 128 ? 64 : 32; }
 
-template <int BN, int STAGES>
+// Elements per k-block: one 128-byte swizzle row, 64 fp16 or 128 e4m3.  Both have the same byte geometry.
+template <bool FP8>
+constexpr int gemm_bk() { return FP8 ? 128 : kGemmBK; }
+
+template <int BN, int STAGES, bool FP8 = false>
 struct GemmSmem {
   static constexpr uint32_t kABytes = kGemmBM * kGemmBK * 2;
   static constexpr uint32_t kBBytes = BN * kGemmBK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;   // multiple of 1024: every operand tile stays swizzle-aligned
-  static constexpr uint32_t kBarOffset = STAGES * kStageBytes;
+  // FP8: the 128 activation scales of each stage's k-block ride the same ring, outside the swizzled operand tiles
+  static constexpr uint32_t kScaleOffset = STAGES * kStageBytes;
+  static constexpr uint32_t kScaleBytes = FP8 ? STAGES * kGemmBM * 4 : 0;
+  static constexpr uint32_t kBarOffset = kScaleOffset + kScaleBytes;
   static constexpr uint32_t kEpiOffset = kBarOffset + 256;     // epilogue staging, one 64 x chunk block per warpgroup
   static constexpr uint32_t kEpiBytes = 2 * 64 * gemm_chunk<BN>() * 4;
-  static constexpr uint32_t kTotal = kEpiOffset + kEpiBytes + 1024;  // alignment slack
+  static constexpr uint32_t kRowScaleOffset = kEpiOffset + kEpiBytes;   // FP8 e4m3 output: 1 / scale of each tile row
+  static constexpr uint32_t kRowScaleBytes = FP8 ? kGemmBM * 4 : 0;
+  static constexpr uint32_t kTotal = kRowScaleOffset + kRowScaleBytes + 1024;  // alignment slack
 };
 
 // Exact-erf GELU (nn.GELU default, vit.py:73).  The epilogue evaluates 63 M of these per MLP layer, so erf uses
@@ -148,6 +169,12 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da
   else wgmma_m64n256k16(acc, da, db, scale_d);
 }
 
+template <int BN>
+__device__ __forceinline__ void wgmma_tile_k32_e4m3(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (BN == 64) wgmma_m64n64k32_e4m3(acc, da, db, scale_d);
+  else wgmma_m64n128k32_e4m3(acc, da, db, scale_d);
+}
+
 __device__ __forceinline__ float gemm_act(int act, float v) {
   return act == kActGelu ? gelu_erf(v) : act == kActRelu ? fmaxf(v, 0.f) : v;
 }
@@ -163,10 +190,13 @@ __device__ __forceinline__ bool aligned16(const void* ptr) { return (reinterpret
 // Staging layout: row r of the chunk holds CH / 4 16-byte units; unit u sits at u ^ swz(r) (low three bits), which keeps
 // both the fragment writes (four rows x 32 bytes per half-warp) and the row reads (eight rows of one unit per
 // quarter-warp) free of bank conflicts.
-template <int BN>
+// FP8 e4m3 output (p.out8): the accumulators already hold act(alpha * acc + bias) (gemm_row_scales_e4m3), so the
+// values are only stored: fp32 / fp16 copies as they are, and the codes of v / s with 1 / s read from row_inv.
+template <int BN, bool FP8 = false>
 __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
                                                    int m0w, int n0, int M_eff, uint32_t bar_id, bool vec_r, bool vec32,
-                                                   bool vec16) {
+                                                   bool vec16, uint32_t row_inv = 0) {
+  const bool final_vals = FP8 && p.out8 != nullptr;
   constexpr int CH = gemm_chunk<BN>();
   constexpr int OCT = CH / 8;          // octets per chunk row
   constexpr int ITEMS = OCT / 2;       // (row, octet) items per thread and chunk: 64 * OCT / 128
@@ -256,13 +286,15 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
         v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
       }
       // alpha * acc + bias + resid, mask, activation: the operation order of the reference epilogue, element for element
+      if (!final_vals) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        v[e] *= p.alpha;
-        if (p.bias) v[e] += bias[k >> 1][e];
-        if (p.resid) v[e] += res[k][e];
-        if (!keep[ri]) v[e] = 0.f;
-        if (p.act32) v[e] = gemm_act(p.act, v[e]);
+        for (int e = 0; e < 8; ++e) {
+          v[e] *= p.alpha;
+          if (p.bias) v[e] += bias[k >> 1][e];
+          if (p.resid) v[e] += res[k][e];
+          if (!keep[ri]) v[e] = 0.f;
+          if (p.act32) v[e] = gemm_act(p.act, v[e]);
+        }
       }
       const bool full = col + 8 <= p.N;
       if (p.out32) {
@@ -276,8 +308,25 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
             if (col + e < p.N) o[e] = v[e];
         }
       }
+      if constexpr (FP8) {
+        if (p.out8) {
+          const float inv = lds_f32(row_inv + 4 * lr);
+          uint8_t* o = p.out8 + static_cast<size_t>(row) * p.ld8 + col;
+          uint16_t q[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) q[e] = cvt_e4m3x2(v[2 * e] * inv, v[2 * e + 1] * inv);
+          if (full && p.ld8 % 8 == 0 && (reinterpret_cast<uintptr_t>(p.out8) & 7) == 0) {
+            *reinterpret_cast<uint2*>(o) = make_uint2(q[0] | (static_cast<uint32_t>(q[1]) << 16),
+                                                      q[2] | (static_cast<uint32_t>(q[3]) << 16));
+          } else {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+              if (col + e < p.N) o[e] = static_cast<uint8_t>(q[e >> 1] >> (8 * (e & 1)));
+          }
+        }
+      }
       if (p.out16) {
-        if (!p.act32) {
+        if (!p.act32 && !final_vals) {
 #pragma unroll
           for (int e = 0; e < 8; ++e) v[e] = gemm_act(p.act, v[e]);
         }
@@ -300,12 +349,47 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
   }
 }
 
-template <int BN, int STAGES, int CLUSTER>
+// e4m3 output, before the element-wise epilogue: replaces the thread's accumulators by v = act(alpha * acc + bias) and
+// derives each tile row's scale from the amax of all its BN = 128 columns (the four lanes of a quad hold one row), so
+// that no code of a row is written before its whole 128-column group has been seen.  The scale goes to out8_scale,
+// its reciprocal (exact: a power of two) to row_inv for the epilogue.
+template <int BN>
+__device__ __forceinline__ void gemm_row_scales_e4m3(const GemmParams& p, float (&acc)[BN / 2], int m0, int n0,
+                                                     int r0, int c0, int wg, int M_eff, uint32_t row_inv) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int col = n0 + 8 * j + c0 + c;
+        float v = acc[4 * j + 2 * i + c] * p.alpha;
+        if (p.bias && col < p.N) v += __ldg(p.bias + col);
+        v = gemm_act(p.act, v);
+        acc[4 * j + 2 * i + c] = v;
+        if (col < p.N) amax = fmaxf(amax, fabsf(v));
+      }
+    }
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+    const float s = e4m3_scale(amax);
+    const int r = r0 + 8 * i;   // row of the tile
+    if ((threadIdx.x & 3) == 0) {
+      sts_f32(row_inv + 4 * (r - wg * 64), 1.0f / s);
+      if (m0 + r < M_eff) p.out8_scale[static_cast<size_t>(n0 / 128) * p.ld8s + m0 + r] = s;
+    }
+  }
+}
+
+template <int BN, int STAGES, int CLUSTER, bool FP8 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using S = GemmSmem<BN, STAGES>;
+  using S = GemmSmem<BN, STAGES, FP8>;
+  constexpr int BK = gemm_bk<FP8>();
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
   static_assert(CLUSTER == 1 || (CLUSTER == 2 && BN >= 128), "cluster pairs split B in two halves of >= 64 rows");
+  static_assert(!FP8 || (CLUSTER == 1 && (BN == 64 || BN == 128)), "FP8: two accumulator sets fit at BN <= 128");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -325,7 +409,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   constexpr int kRows = kGemmBM * CLUSTER;   // rows of one tile of the CTA (cluster)
   const int tiles_m = (M_eff + kRows - 1) / kRows;
   const int tiles_n = (p.N + BN - 1) / BN;
-  const int num_kb = (p.K + kGemmBK - 1) / kGemmBK;
+  const int num_kb = (p.K + BK - 1) / BK;
   const bool m_stationary = p.argmin_out != nullptr;   // (the host never combines arg-min with CLUSTER = 2)
   const int rank = CLUSTER == 2 ? static_cast<int>(cluster_ctarank()) : 0;
   const int tile0 = static_cast<int>(blockIdx.x) / CLUSTER, tile_step = static_cast<int>(gridDim.x) / CLUSTER;
@@ -362,12 +446,15 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           const int tap = kb / p.kblocks_per_tap;
           const int kk = kb - tap * p.kblocks_per_tap;
           // the whole stage lands here: own A rows, own half of B and (CLUSTER = 2) the peer's half of B
-          mbar_arrive_expect_tx(&full_bar[stage], S::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kk * kGemmBK, m0 + p.tap_row0 + tap * p.tap_stride);
+          mbar_arrive_expect_tx(&full_bar[stage], S::kStageBytes + (FP8 ? kGemmBM * 4 : 0));
+          tma_load_2d(sa, &tmA, &full_bar[stage], kk * BK, m0 + p.tap_row0 + tap * p.tap_stride);
           if constexpr (CLUSTER == 2)
-            tma_load_2d_mcast(sb + rank * (BN / 2) * 128, &tmB, &full_bar[stage], kb * kGemmBK, n0 + rank * (BN / 2), 3);
+            tma_load_2d_mcast(sb + rank * (BN / 2) * 128, &tmB, &full_bar[stage], kb * BK, n0 + rank * (BN / 2), 3);
           else
-            tma_load_2d(sb, &tmB, &full_bar[stage], kb * kGemmBK, n0);
+            tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n0);
+          if constexpr (FP8)
+            bulk_load_1d(smem + S::kScaleOffset + stage * kGemmBM * 4, p.a_scale + static_cast<size_t>(kb) * p.ld_as + m0,
+                         kGemmBM * 4, &full_bar[stage]);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -395,6 +482,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   int stage = 0;
   uint32_t phase = 0;
   float acc[BN / 2];
+  float tile[FP8 ? BN / 2 : 1];   // FP8: the current k-block's products
 
   // a consumed stage is released to the producers of every CTA of the cluster
   auto release = [&](int s) {
@@ -412,27 +500,57 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     const int m0 = it.m0(kRows) + rank * kGemmBM;
     const int n0 = it.n0(BN);
     int prev = -1;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_base + stage * S::kStageBytes + wg * (64 * 128);
-      const uint32_t sb = smem_base + stage * S::kStageBytes + S::kABytes;
-      wgmma_fence_operand(acc);
-      wgmma_fence();
+    if constexpr (FP8) {
+      // per k-block: four k32 MMAs into a fresh tile, then the promotion  acc += tile * (s_a[row] * s_w).  The tile is
+      // reused by the next k-block, so each warpgroup waits for its MMAs; the other warpgroup's keep the tensor core busy.
+      const int r0l = r0 - wg * 64;
+      const float* wsc = p.w_scale + static_cast<size_t>(n0 / 128) * num_kb;
 #pragma unroll
-      for (int k = 0; k < kGemmBK / 16; ++k)
-        wgmma_tile_k16<BN>(acc, make_wgmma_desc_sw128(sa + k * 32), make_wgmma_desc_sw128(sb + k * 32),
-                           (kb | k) != 0 ? 1u : 0u);
-      wgmma_commit();
-      // the previous k-block's MMAs have retired once at most one group is pending: its smem slot is free
-      wgmma_wait<1>();
+      for (int a = 0; a < BN / 2; ++a) acc[a] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_base + stage * S::kStageBytes + wg * (64 * 128);
+        const uint32_t sb = smem_base + stage * S::kStageBytes + S::kABytes;
+        wgmma_fence_operand(tile);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 32; ++k)
+          wgmma_tile_k32_e4m3<BN>(tile, make_wgmma_desc_sw128(sa + k * 32), make_wgmma_desc_sw128(sb + k * 32),
+                                  k != 0 ? 1u : 0u);
+        wgmma_commit();
+        const float sw = __ldg(wsc + kb);
+        const uint32_t ss = smem_base + S::kScaleOffset + stage * kGemmBM * 4 + (wg * 64 + r0l) * 4;
+        const float s0 = lds_f32(ss) * sw, s1 = lds_f32(ss + 32) * sw;   // rows r0, r0 + 8: exact products
+        wgmma_wait<0>();
+        wgmma_fence_operand(tile);
+        release(stage);
+#pragma unroll
+        for (int a = 0; a < BN / 2; ++a) acc[a] = fmaf(tile[a], (a & 2) ? s1 : s0, acc[a]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    } else {
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_base + stage * S::kStageBytes + wg * (64 * 128);
+        const uint32_t sb = smem_base + stage * S::kStageBytes + S::kABytes;
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kGemmBK / 16; ++k)
+          wgmma_tile_k16<BN>(acc, make_wgmma_desc_sw128(sa + k * 32), make_wgmma_desc_sw128(sb + k * 32),
+                             (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        // the previous k-block's MMAs have retired once at most one group is pending: its smem slot is free
+        wgmma_wait<1>();
+        wgmma_fence_operand(acc);
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
       wgmma_fence_operand(acc);
       if (prev >= 0) release(prev);
-      prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-    wgmma_wait<0>();
-    wgmma_fence_operand(acc);
-    if (prev >= 0) release(prev);
 
     if (p.argmin_out) {
       // ---- row arg-min: running (best, index[, second]) of the thread's two rows over its columns, in column order
@@ -496,6 +614,10 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           best_idx[i] = 0;
         }
       }
+    } else if constexpr (FP8) {
+      const uint32_t row_inv = smem_base + S::kRowScaleOffset + wg * 64 * 4;
+      if (p.out8) gemm_row_scales_e4m3<BN>(p, acc, m0, n0, r0, c0, wg, M_eff, row_inv);
+      gemm_epilogue_rows<BN, true>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16, row_inv);
     } else {
       gemm_epilogue_rows<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16);
     }

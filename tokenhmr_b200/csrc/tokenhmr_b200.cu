@@ -38,7 +38,7 @@ int dev_clone(T** p, const T* src, size_t n) {
 
 extern "C" {
 
-int thmr_abi_version(void) { return 5; }
+int thmr_abi_version(void) { return 6; }
 
 const char* thmr_last_error(void) { return last_error_buf(); }
 
@@ -605,14 +605,20 @@ int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr
   THMR_CHECK(maxdil <= kTokPad, "engine_create: dilation %d exceeds sequence padding %d", maxdil, kTokPad);
   THMR_CHECK(smpl->m.nb <= 10 && smpl->m.n_extra + 25 <= 64, "engine_create: SMPL model shape");
   THMR_CHECK(w->blocks_host && w->dec_host && w->mixer_host, "engine_create: missing layer arrays");
+  THMR_CHECK(!(cfg->strict && cfg->fp8), "engine_create: strict and fp8 are exclusive numeric modes");
+  THMR_CHECK(!cfg->fp8 || w->block_scales_host, "engine_create: fp8 needs the weights' block scales");
+  THMR_CHECK(!cfg->fp8 || (cfg->vit_dim % 128 == 0 && (cfg->vit_dim == 1280 || cfg->vit_dim == 1024 ||
+                                                       cfg->vit_dim == 128)),
+             "engine_create: fp8 needs vit_dim 128, 1024 or 1280 (e4m3 LayerNorm widths)");
   thmr_engine* e = new (std::nothrow) thmr_engine();
   if (!e) return fail(THMR_ERR_NOMEM, "engine_create: out of host memory");
   e->cfg = *cfg;
   e->w = *w;
   e->blocks.assign(w->blocks_host, w->blocks_host + cfg->vit_depth);
+  if (cfg->fp8) e->block_scales.assign(w->block_scales_host, w->block_scales_host + cfg->vit_depth);
   e->dec.assign(w->dec_host, w->dec_host + cfg->dec_depth);
   e->mixer.assign(w->mixer_host, w->mixer_host + cfg->cls_blocks);
-  e->w.blocks_host = nullptr; e->w.dec_host = nullptr; e->w.mixer_host = nullptr;
+  e->w.blocks_host = nullptr; e->w.dec_host = nullptr; e->w.mixer_host = nullptr; e->w.block_scales_host = nullptr;
   e->smpl = smpl;
   *out = e;
   return THMR_OK;

@@ -53,7 +53,7 @@ class TokenHMREngine(nn.Module):
     def __init__(self, cfg: TokenHMRConfig, state_dict: Dict[str, torch.Tensor], smpl: Dict[str, torch.Tensor],
                  device: str | torch.device = "cuda:0", max_batch: int = 256, use_cuda_graph: bool = True,
                  strict: bool = False, alias_outputs: bool = False, max_cached_shapes: int = 6,
-                 concurrent: bool = False):
+                 concurrent: bool = False, fp8: bool = False):
         """strict: every contraction of the path in split-fp16 (3 tensor-core products, ~2^-21 relative: fp32-grade)
         instead of fp16 operands -- the mode whose results match the fp32 reference to 1e-4 with identical pose tokens
         (DESIGN.md §2); about 4x slower.  alias_outputs: return views of the engine's static output buffers (valid until
@@ -62,7 +62,11 @@ class TokenHMREngine(nn.Module):
         buffer sets kept alive; the least recently used one is dropped beyond that.
         concurrent: the forwards of different slots may run at the same time on different streams
         (TokenHMRPipeline(streams=2)); the engine then avoids kernels that need the whole GPU to themselves
-        (thmr_config::concurrent)."""
+        (thmr_config::concurrent).
+        fp8: the ViT's QKV, fc1 and fc2 GEMMs (88 % of the model's FLOPs) run on block-scaled e4m3 operands on the FP8
+        tensor cores (thmr_config::fp8, DESIGN.md §2 for its accuracy); not with strict."""
+        if strict and fp8:
+            raise _lib.ThmrError("strict and fp8 are exclusive numeric modes")
         super().__init__()
         self.cfg = cfg
         self.device = torch.device(device)
@@ -75,13 +79,15 @@ class TokenHMREngine(nn.Module):
         validate_against_weights(cfg, state_dict, smpl)
         self.strict = bool(strict)
         self.concurrent = bool(concurrent)
+        self.fp8 = bool(fp8)
         self.alias_outputs = bool(alias_outputs)
         self.max_cached_shapes = int(max_cached_shapes)
         with torch.cuda.device(self.device):
-            self.weights = PackedWeights(state_dict, cfg, self.device, strict=self.strict)
+            self.weights = PackedWeights(state_dict, cfg, self.device, strict=self.strict, fp8=self.fp8)
             self.smpl_model = SMPLModel(smpl, self.device)
             self.smpl = _SmplFacade(self.smpl_model)
-            self._cfg_struct = make_config_struct(cfg, strict=self.strict, concurrent=self.concurrent)
+            self._cfg_struct = make_config_struct(cfg, strict=self.strict, concurrent=self.concurrent,
+                                                  fp8=self.fp8)
             h = ctypes.c_void_p()
             check(lib().thmr_engine_create(ctypes.byref(self._cfg_struct), ctypes.byref(self.weights.struct),
                                            self.smpl_model.handle, ctypes.byref(h)))

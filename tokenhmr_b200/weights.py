@@ -16,6 +16,7 @@ from typing import Dict, List
 import torch
 
 from . import _lib
+from . import fp8 as _fp8
 from .config import TokenHMRConfig
 
 
@@ -55,12 +56,18 @@ def split_weight(t: torch.Tensor, taps: int = 1) -> torch.Tensor:
 class PackedWeights:
     """Owns the device tensors the engine points into (must outlive the engine)."""
 
-    def __init__(self, sd: Dict[str, torch.Tensor], cfg: TokenHMRConfig, device: torch.device, strict: bool = False):
+    def __init__(self, sd: Dict[str, torch.Tensor], cfg: TokenHMRConfig, device: torch.device, strict: bool = False,
+                 fp8: bool = False):
         """strict: matrices are packed for the split-fp16 GEMMs of strict mode (csrc/strict.cuh): f16 [out, 3*in] =
-        [hi | hi | lo] of w * 2^8 with hi = fp16(w * 2^8), lo = fp16(w * 2^8 - hi); conv weights per tap."""
+        [hi | hi | lo] of w * 2^8 with hi = fp16(w * 2^8), lo = fp16(w * 2^8 - hi); conv weights per tap.
+        fp8: each ViT block's qkv, fc1 and fc2 weights are e4m3 [out, in] codes with one power-of-two scale per
+        128 x 128 block (tokenhmr_b200/fp8.py, quantised from fp32 on the device); everything else as by default."""
+        if strict and fp8:
+            raise _lib.ThmrError("strict and fp8 are exclusive numeric modes")
         self.cfg = cfg
         self.device = device
         self.strict = bool(strict)
+        self.fp8 = bool(fp8)
         self._keep: List[torch.Tensor] = []
         g = lambda n: sd[n]
 
@@ -71,6 +78,15 @@ class PackedWeights:
                 t = t.detach().to(device=device, dtype=torch.float16).contiguous()
             self._keep.append(t)
             return t.data_ptr()
+
+        def vit_w(t: torch.Tensor, i: int, scale_field: str) -> int:
+            """A ViT GEMM weight that the FP8 mode runs on e4m3: its codes, with the block scales recorded."""
+            if not self.fp8:
+                return f16(t)
+            codes, scales = _fp8.quantize_weight_blocks(t.detach().to(device=device, dtype=torch.float32))
+            self._keep += [codes, scales]
+            setattr(self.block_scales[i], scale_field, scales.data_ptr())
+            return codes.data_ptr()
 
         def f32(t: torch.Tensor) -> int:
             t = t.detach().to(device=device, dtype=torch.float32).contiguous()
@@ -91,16 +107,19 @@ class PackedWeights:
         pos = g("backbone.pos_embed")
         W.pos = f32(pos[0, 1:] + pos[0, :1])               # vit.py:327
         self.blocks = (_lib.VitBlock * cfg.vit_depth)()
+        self.block_scales = (_lib.VitBlockScales * cfg.vit_depth)()
         for i in range(cfg.vit_depth):
             p = f"backbone.blocks.{i}."
             b = self.blocks[i]
             b.ln1_g, b.ln1_b = f32(g(p + "norm1.weight")), f32(g(p + "norm1.bias"))
-            b.qkv_w, b.qkv_b = f16(g(p + "attn.qkv.weight")), f32(g(p + "attn.qkv.bias"))
+            b.qkv_w, b.qkv_b = vit_w(g(p + "attn.qkv.weight"), i, "qkv_ws"), f32(g(p + "attn.qkv.bias"))
             b.proj_w, b.proj_b = f16(g(p + "attn.proj.weight")), f32(g(p + "attn.proj.bias"))
             b.ln2_g, b.ln2_b = f32(g(p + "norm2.weight")), f32(g(p + "norm2.bias"))
-            b.fc1_w, b.fc1_b = f16(g(p + "mlp.fc1.weight")), f32(g(p + "mlp.fc1.bias"))
-            b.fc2_w, b.fc2_b = f16(g(p + "mlp.fc2.weight")), f32(g(p + "mlp.fc2.bias"))
+            b.fc1_w, b.fc1_b = vit_w(g(p + "mlp.fc1.weight"), i, "fc1_ws"), f32(g(p + "mlp.fc1.bias"))
+            b.fc2_w, b.fc2_b = vit_w(g(p + "mlp.fc2.weight"), i, "fc2_ws"), f32(g(p + "mlp.fc2.bias"))
         W.blocks_host = ctypes.cast(self.blocks, ctypes.POINTER(_lib.VitBlock))
+        if self.fp8:
+            W.block_scales_host = ctypes.cast(self.block_scales, ctypes.POINTER(_lib.VitBlockScales))
         W.last_g, W.last_b = f32(g("backbone.last_norm.weight")), f32(g("backbone.last_norm.bias"))
         # ---- decoder
         t = "smpl_head.transformer."
@@ -167,10 +186,14 @@ class PackedWeights:
         return sum(t.numel() * t.element_size() for t in self._keep)
 
 
-def make_config_struct(cfg: TokenHMRConfig, strict: bool = False, concurrent: bool = False) -> _lib.Config:
+def make_config_struct(cfg: TokenHMRConfig, strict: bool = False, concurrent: bool = False,
+                       fp8: bool = False) -> _lib.Config:
+    if strict and fp8:
+        raise _lib.ThmrError("strict and fp8 are exclusive numeric modes")
     c = _lib.Config()
     c.strict = 1 if strict else 0
     c.concurrent = 1 if concurrent else 0
+    c.fp8 = 1 if fp8 else 0
     for f in ("image_size", "crop_w", "patch", "patch_pad", "vit_dim", "vit_depth", "vit_heads", "vit_mlp_ratio",
               "vit_ln_eps", "dec_dim", "dec_depth", "dec_heads", "dec_dim_head", "dec_mlp_dim", "ln_eps", "token_num",
               "token_class_num", "cls_hidden", "cls_hidden_inter", "cls_token_inter", "cls_blocks", "code_dim",
