@@ -1,14 +1,17 @@
 // Test-only probe library (tests/libthmr_probe.so): thin extern "C" wrappers around the launchers of
 // tokenhmr_b200/csrc that the engine dispatches but the product ABI does not expose (GEMM epilogue options, the
 // split-precision operand builder, the strict-mode fp32 kernels, the head and tokenizer glue kernels, every LayerNorm
-// dispatch variant).  Each wrapper launches exactly what the engine launches, with the engine's grid shapes, so that
-// tests/test_gpu_kernels.py and tests/test_gpu_strict_kernels.py can compare one stage at a time against fp64.
+// dispatch variant, the SMPL stage's kernels).  Each wrapper launches exactly what the engine launches, with the engine's
+// grid shapes, so that tests/test_gpu_kernels.py, tests/test_gpu_strict_kernels.py and tests/test_gpu_smpl_kernels.py can
+// compare one stage at a time against fp64.
 // The product never loads this library.
 #include "../../tokenhmr_b200/csrc/attention_mma.cuh"
 #include "../../tokenhmr_b200/csrc/common.cuh"
 #include "../../tokenhmr_b200/csrc/elementwise.cuh"
+#include "../../tokenhmr_b200/csrc/engine.cuh"
 #include "../../tokenhmr_b200/csrc/gemm_host.cuh"
 #include "../../tokenhmr_b200/csrc/head_kernels.cuh"
+#include "../../tokenhmr_b200/csrc/smpl_lbs.cuh"
 #include "../../tokenhmr_b200/csrc/strict.cuh"
 
 using namespace thmr;
@@ -162,5 +165,78 @@ PROBE_API int probe_head_assemble(const float* readout, int ld_r, const float* b
   head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, as_stream(stream)>>>(readout, ld_r, bpose, ld_b, pitch, lo,
                                                                            init_pose, init_betas, init_cam, rotmats,
                                                                            betas, cam, pose6d, B, nb);
+  PROBE_LAUNCHED();
+}
+
+// ---- SMPL stage (smpl_lbs.cuh; launched by thmr_smpl_create and smpl_run in engine.cuh) --------------------------
+// thmr_smpl_create: J_template / J_shapedirs, one block per output scalar
+PROBE_API int probe_smpl_jreg(const float* Jreg, const float* v_template, const float* shapedirs, float* J_template,
+                              float* J_shapedirs, int V, int nb, void* stream) {
+  smpl_jreg_kernel<<<kSmplJ * 3 * (nb + 1), 256, 0, as_stream(stream)>>>(Jreg, v_template, shapedirs, J_template,
+                                                                         J_shapedirs, V, nb);
+  PROBE_LAUNCHED();
+}
+
+// thmr_smpl_create: zero the basis including its pad rows (3V rounded up to 4), then pack [3V, 3*224]
+PROBE_API int probe_smpl_pack_posedirs(const float* posedirs, const float* shapedirs, const float* v_template, int nb,
+                                       void* out, int V, void* stream) {
+  const size_t rows_pad = (static_cast<size_t>(3) * V + 3) / 4 * 4;
+  THMR_CUDA(cudaMemsetAsync(out, 0, rows_pad * 3 * kSmplPFPad * sizeof(__half), as_stream(stream)));
+  const long n = static_cast<long>(3) * V * kSmplPFPad;
+  smpl_pack_posedirs_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, as_stream(stream)>>>(
+      posedirs, shapedirs, v_template, nb, static_cast<__half*>(out), 3 * V);
+  PROBE_LAUNCHED();
+}
+
+PROBE_API int probe_smpl_pose(const float* pose, int pose2rot, const float* betas, const float* J_template,
+                              const float* J_shapedirs, int nb, const int* parents_dev, float* A, float* Jposed,
+                              void* pf16, int B, void* stream) {
+  smpl_pose_kernel<<<B, 32, 0, as_stream(stream)>>>(pose, pose2rot, betas, J_template, J_shapedirs, nb, parents_dev, A,
+                                                    Jposed, static_cast<__half*>(pf16), B);
+  PROBE_LAUNCHED();
+}
+
+// The blend GEMM of one chunk of n poses starting at pose p0, planned by smpl_blend_plan as smpl_run does:
+// pf16 [>= p0 + n, 3*224], posedirsT [off_pitch, 3*224], offsets [n, off_pitch] with off_pitch = 3V rounded up to 4.
+PROBE_API int probe_smpl_blend(const void* pf16, const void* posedirsT, int V, int p0, int n, float* offsets,
+                               void* stream) {
+  SmplModel m;
+  m.V = V;
+  m.posedirsT = static_cast<__half*>(const_cast<void*>(posedirsT));
+  SmplWs ws{};
+  ws.pf16 = static_cast<__half*>(const_cast<void*>(pf16));
+  ws.offsets = offsets;
+  ws.off_pitch = (3L * V + 3) / 4 * 4;   // smpl_carve
+  GemmPlan plan;
+  THMR_TRY(smpl_blend_plan(m, ws, p0, n, &plan));
+  return gemm_launch(plan, as_stream(stream));
+}
+
+// smpl_run's skinning launch; threads (256 | 128) and ell_reg (4 | 8) pick the instantiation
+PROBE_API int probe_smpl_skin(int threads, int ell_reg, const int* w_idx, const float* w_val, int ell, const float* A,
+                              const float* vposed, long off_pitch, float* verts, long vert_pitch, int V, int B,
+                              void* stream) {
+  THMR_CHECK((threads == 256 || threads == 128) && (ell_reg == 4 || ell_reg == 8), "probe_smpl_skin: threads %d ell_reg %d",
+             threads, ell_reg);
+  const dim3 grid((V + threads - 1) / threads, (B + kSkinPoses - 1) / kSkinPoses);
+  cudaStream_t st = as_stream(stream);
+  if (threads == 256 && ell_reg == 4)
+    smpl_skin_kernel<256, 4><<<grid, 256, 0, st>>>(w_idx, w_val, ell, A, vposed, off_pitch, verts, vert_pitch, V, B);
+  else if (threads == 256)
+    smpl_skin_kernel<256, 8><<<grid, 256, 0, st>>>(w_idx, w_val, ell, A, vposed, off_pitch, verts, vert_pitch, V, B);
+  else if (ell_reg == 4)
+    smpl_skin_kernel<128, 4><<<grid, 128, 0, st>>>(w_idx, w_val, ell, A, vposed, off_pitch, verts, vert_pitch, V, B);
+  else
+    smpl_skin_kernel<128, 8><<<grid, 128, 0, st>>>(w_idx, w_val, ell, A, vposed, off_pitch, verts, vert_pitch, V, B);
+  PROBE_LAUNCHED();
+}
+
+PROBE_API int probe_smpl_joints(const float* Jposed, const float* verts, long vert_pitch, const int* joint_map,
+                                const int* extra_vid, const int* jx_ptr, const int* jx_idx, const float* jx_val,
+                                int n_extra, float* joints, const float* pred_cam, float focal, float image_size,
+                                float* cam_t, float* focal_out, float* kp2d, int B, void* stream) {
+  smpl_joints_kernel<<<B, 64, 0, as_stream(stream)>>>(Jposed, verts, vert_pitch, joint_map, extra_vid, jx_ptr, jx_idx,
+                                                      jx_val, n_extra, joints, pred_cam, focal, image_size, cam_t,
+                                                      focal_out, kp2d);
   PROBE_LAUNCHED();
 }

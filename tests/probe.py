@@ -46,6 +46,12 @@ SIGNATURES = {
     "probe_mixer_add": (c_int, [P, P, P, P, I, I, I, P]),
     "probe_cast_f16": (c_int, [P, P, L, P]),
     "probe_head_assemble": (c_int, [P, I, P, I, I, I, P, P, P, P, P, P, P, I, I, P]),
+    "probe_smpl_jreg": (c_int, [P, P, P, P, P, I, I, P]),
+    "probe_smpl_pack_posedirs": (c_int, [P, P, P, I, P, I, P]),
+    "probe_smpl_pose": (c_int, [P, I, P, P, P, I, P, P, P, P, I, P]),
+    "probe_smpl_blend": (c_int, [P, P, I, I, I, P, P]),
+    "probe_smpl_skin": (c_int, [I, I, P, P, I, P, P, L, P, L, I, I, P]),
+    "probe_smpl_joints": (c_int, [P, P, L, P, P, P, P, P, I, P, P, F, F, P, P, P, I, P]),
 }
 
 ACT = {"none": 0, "gelu": 1, "relu": 2}      # kActNone / kActGelu / kActRelu == kSplitAct*
