@@ -212,6 +212,71 @@ size_t thmr_tok_encoder_workspace_bytes(const thmr_tok_encoder* e, int batch);
 int thmr_tok_encode(const thmr_tok_encoder* e, const float* pose6d, int B, int64_t* code_idx, float* latent,
                     void* workspace, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Mesh rendering: the reference's Renderer.__call__ / render_rgba_multiple [tokenhmr/lib/utils/renderer.py:137-359]
+ * as a rasterizer (DESIGN.md §2 "Rendering": geometry pinned to the reference's camera chain, shading a stated model).
+ * Frame: the model's camera frame (x right, y down, z forward).  A vertex v of mesh i lands at
+ *   q = R v + t_i (rotate_translation = 0: Renderer.__call__, R = the side-view rotation or I)  or
+ *   q = R (v + t_i) (rotate_translation = 1: render_rgba_multiple, R = its rot_axis / rot_angle rotation),
+ * and pixel (c, r) holds what covers the point (focal q.x / q.z + W/2, focal q.y / q.z + H/2) = (c + 0.5, r + 0.5).
+ * ---------------------------------------------------------------------------------------------- */
+#define THMR_RENDER_MAX_LIGHTS 16
+#define THMR_RENDER_MAX_MESHES 1024
+enum { THMR_LIGHT_DIRECTIONAL = 0, THMR_LIGHT_POINT = 1 };
+enum { THMR_BG_NONE = 0, THMR_BG_HWC = 1, THMR_BG_CHW_NORMALIZED = 2 };
+
+/* The faces of a mesh, checked and indexed once: every index must lie in [0, num_verts) (THMR_ERR_INVALID otherwise),
+ * and a vertex -> face list is built so that smooth normals are gathered in a fixed order (bitwise stable).
+ * faces_host int32 [F,3] HOST.  Synchronous (uploads to engine-owned device memory). */
+typedef struct thmr_render_topology thmr_render_topology;
+int thmr_render_topology_create(const int32_t* faces_host, int num_faces, int num_verts, thmr_render_topology** out);
+void thmr_render_topology_destroy(thmr_render_topology* t);
+
+typedef struct thmr_render_light {
+  int type;         /* THMR_LIGHT_DIRECTIONAL: vec = unit direction towards the light;  THMR_LIGHT_POINT: vec = position */
+  float vec[3];     /* camera frame (x right, y down, z forward) */
+  float intensity;  /* white light */
+} thmr_render_light;
+
+typedef struct thmr_render_desc {
+  const thmr_render_topology* topology;
+  int n_meshes;                   /* 1 .. THMR_RENDER_MAX_MESHES */
+  int n_images;                   /* >= 1 */
+  const int32_t* mesh_image_host; /* HOST [n_meshes]: image of each mesh, each in [0, n_images); NULL = mesh i -> image i */
+  const float* vertices;          /* [n_meshes, V, 3] */
+  const float* translations;      /* [n_meshes, 3] */
+  float rotation[9];              /* R, row-major */
+  int rotate_translation;         /* 0: q = R v + t;  1: q = R (v + t) */
+  int width, height;              /* image size in pixels, each 1 .. 16384 */
+  float focal;                    /* fx = fy, > 0 */
+  float znear;                    /* faces with a vertex at q.z < znear are dropped, not clipped (pyrender default 0.05) */
+  float base_color[3];            /* mesh colour, 0..1 */
+  float bg_color[3];              /* colour of uncovered pixels, alpha 0 */
+  float ambient;                  /* 0.3 in the reference */
+  int n_lights;                   /* 0 .. THMR_RENDER_MAX_LIGHTS */
+  thmr_render_light lights[THMR_RENDER_MAX_LIGHTS];
+  int bg_layout;                  /* image under the composite: THMR_BG_HWC fp32 [n_images, H, W, 3], or
+                                   * THMR_BG_CHW_NORMALIZED fp32 [n_images, 3, H, W] shown as img * std + mean */
+  const float* bg_image;
+  float mean[3], std[3];          /* THMR_BG_CHW_NORMALIZED only */
+  /* outputs, each nullable, [n_images, H, W, ...] fp32 unless stated:
+   * rgba [.., 4] (alpha = coverage; 16-byte aligned, THMR_ERR_INVALID otherwise), composite [.., 3] = rgb * alpha + (1 - alpha) * image (needs bg_layout != NONE),
+   * face_id int32 [..] (mesh * F + face, -1 where uncovered), depth [..] (camera-frame z, 0 where uncovered) */
+  float* rgba;
+  float* composite;
+  int32_t* face_id;
+  float* depth;
+} thmr_render_desc;
+
+/* Workspace of one thmr_render_meshes call (pure arithmetic). */
+size_t thmr_render_workspace_bytes(const thmr_render_topology* t, int n_meshes, int n_images, int width, int height);
+/* Renders every mesh of the desc.  Stream-ordered, no host synchronisation, no allocation: CUDA-graph capturable (a
+ * captured call keeps the desc's scalar fields and host arrays as they were when captured).  Returns
+ * THMR_ERR_INVALID, with nothing launched, for a null topology / vertices / translations / workspace, sizes out of
+ * range, an image index out of range, a light type other than the two above, a composite without an image, or a
+ * misaligned rgba. */
+int thmr_render_meshes(const thmr_render_desc* desc, void* workspace, void* stream);
+
 /* ================================================================================================
  * Engine: TokenHMR.forward(batch)  [tokenhmr.py:330-338 -> 135-188]
  * ============================================================================================== */

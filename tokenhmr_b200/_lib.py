@@ -92,6 +92,26 @@ class PreprocCfg(Structure):
                 ("mean", ctypes.c_double * 3), ("std", ctypes.c_double * 3)]
 
 
+RENDER_MAX_LIGHTS = 16
+RENDER_MAX_MESHES = 1024
+LIGHT_DIRECTIONAL, LIGHT_POINT = 0, 1
+BG_NONE, BG_HWC, BG_CHW_NORMALIZED = 0, 1, 2
+
+
+class RenderLight(Structure):
+    _fields_ = [("type", c_int), ("vec", c_float * 3), ("intensity", c_float)]
+
+
+class RenderDesc(Structure):
+    _fields_ = [("topology", c_void_p), ("n_meshes", c_int), ("n_images", c_int), ("mesh_image_host", POINTER(c_int32)),
+                ("vertices", c_void_p), ("translations", c_void_p), ("rotation", c_float * 9),
+                ("rotate_translation", c_int), ("width", c_int), ("height", c_int), ("focal", c_float),
+                ("znear", c_float), ("base_color", c_float * 3), ("bg_color", c_float * 3), ("ambient", c_float),
+                ("n_lights", c_int), ("lights", RenderLight * RENDER_MAX_LIGHTS), ("bg_layout", c_int),
+                ("bg_image", c_void_p), ("mean", c_float * 3), ("std", c_float * 3),
+                ("rgba", c_void_p), ("composite", c_void_p), ("face_id", c_void_p), ("depth", c_void_p)]
+
+
 class Outputs(Structure):
     _fields_ = [(n, c_void_p) for n in ("cls_logits_softmax", "pred_cam", "rotmats", "betas", "pred_cam_t",
                                         "focal_length", "pred_keypoints_3d", "pred_vertices", "pred_keypoints_2d",
@@ -146,6 +166,10 @@ SIGNATURES = {
     "thmr_tok_encoder_num_tokens": (c_int, [c_void_p]),
     "thmr_tok_encoder_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "thmr_tok_encode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "thmr_render_topology_create": (c_int, [c_void_p, c_int, c_int, POINTER(c_void_p)]),
+    "thmr_render_topology_destroy": (None, [c_void_p]),
+    "thmr_render_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
+    "thmr_render_meshes": (c_int, [POINTER(RenderDesc), c_void_p, c_void_p]),
     "thmr_smpl_create": (c_int, [POINTER(SmplDesc), POINTER(c_void_p)]),
     "thmr_smpl_destroy": (None, [c_void_p]),
     "thmr_smpl_workspace_bytes": (c_size_t, [c_void_p, c_int]),

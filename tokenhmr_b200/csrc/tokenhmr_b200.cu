@@ -9,6 +9,7 @@
 #include "engine_strict.cuh"
 #include "eval_kernels.cuh"
 #include "preproc.cuh"
+#include "render.cuh"
 #include "tok_encoder.cuh"
 
 using namespace thmr;
@@ -38,7 +39,7 @@ int dev_clone(T** p, const T* src, size_t n) {
 
 extern "C" {
 
-int thmr_abi_version(void) { return 6; }
+int thmr_abi_version(void) { return 7; }
 
 const char* thmr_last_error(void) { return last_error_buf(); }
 
@@ -447,6 +448,108 @@ int thmr_tok_encode(const thmr_tok_encoder* e, const float* pose6d, int B, int64
   THMR_CHECK(B > 0, "tok_encode: bad batch %d", B);
   void* ws = reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
   return enc_run(e, pose6d, B, code_idx, latent, ws, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------ rendering
+void thmr_render_topology_destroy(thmr_render_topology* t) {
+  if (!t) return;
+  cudaFree(t->faces); cudaFree(t->vf_off); cudaFree(t->vf_face);
+  delete t;
+}
+
+int thmr_render_topology_create(const int32_t* faces_host, int F, int V, thmr_render_topology** out) {
+  THMR_CHECK(faces_host && out, "render_topology_create: null argument");
+  THMR_CHECK(F > 0 && V > 0 && F <= (1 << 26) && V <= (1 << 26), "render_topology_create: F=%d V=%d", F, V);
+  std::vector<int32_t> off(static_cast<size_t>(V) + 1, 0), vf(3 * static_cast<size_t>(F));
+  for (size_t k = 0; k < 3 * static_cast<size_t>(F); ++k) {
+    const int32_t i = faces_host[k];
+    THMR_CHECK(i >= 0 && i < V, "render_topology_create: face %zu has vertex index %d outside [0, %d)", k / 3, i, V);
+    ++off[i + 1];
+  }
+  for (int i = 0; i < V; ++i) off[i + 1] += off[i];
+  std::vector<int32_t> fill(off.begin(), off.end() - 1);
+  for (int f = 0; f < F; ++f)   // ascending face order within every vertex's list
+    for (int c = 0; c < 3; ++c) vf[fill[faces_host[3 * f + c]]++] = f;
+  thmr_render_topology* t = new (std::nothrow) thmr_render_topology();
+  THMR_CHECK(t, "render_topology_create: out of host memory");
+  t->F = F; t->V = V;
+  std::vector<int32_t> fh(faces_host, faces_host + 3 * static_cast<size_t>(F));
+  int s = dev_upload(&t->faces, fh);
+  if (s == THMR_OK) s = dev_upload(&t->vf_off, off);
+  if (s == THMR_OK) s = dev_upload(&t->vf_face, vf);
+  if (s != THMR_OK) { thmr_render_topology_destroy(t); return s; }
+  *out = t;
+  return THMR_OK;
+}
+
+size_t thmr_render_workspace_bytes(const thmr_render_topology* t, int n_meshes, int n_images, int width, int height) {
+  if (!t || n_meshes <= 0 || n_images <= 0 || width <= 0 || height <= 0) return 0;
+  return render_carve(nullptr, t->V, n_meshes, n_images, width, height, nullptr) + 1024;
+}
+
+int thmr_render_meshes(const thmr_render_desc* d, void* workspace, void* stream) {
+  THMR_CHECK(d && workspace, "render_meshes: null desc or workspace");
+  const thmr_render_topology* t = d->topology;
+  THMR_CHECK(t && d->vertices && d->translations, "render_meshes: null topology, vertices or translations");
+  THMR_CHECK(d->n_meshes >= 1 && d->n_meshes <= THMR_RENDER_MAX_MESHES, "render_meshes: n_meshes %d (1 .. %d)",
+             d->n_meshes, THMR_RENDER_MAX_MESHES);
+  THMR_CHECK(d->n_images >= 1, "render_meshes: n_images %d", d->n_images);
+  THMR_CHECK(d->width >= 1 && d->width <= 16384 && d->height >= 1 && d->height <= 16384, "render_meshes: size %dx%d",
+             d->width, d->height);
+  THMR_CHECK(static_cast<long long>(d->n_meshes) * t->F < (1ll << 31), "render_meshes: n_meshes * F overflows face ids");
+  THMR_CHECK(static_cast<long long>(d->n_images) * d->width * d->height <= (1ll << 34), "render_meshes: too many pixels");
+  THMR_CHECK(d->focal > 0.f && isfinite(d->focal), "render_meshes: focal %g", d->focal);
+  THMR_CHECK(d->znear > 0.f && isfinite(d->znear), "render_meshes: znear %g", d->znear);
+  THMR_CHECK(d->n_lights >= 0 && d->n_lights <= THMR_RENDER_MAX_LIGHTS, "render_meshes: n_lights %d", d->n_lights);
+  for (int l = 0; l < d->n_lights; ++l)
+    THMR_CHECK(d->lights[l].type == THMR_LIGHT_DIRECTIONAL || d->lights[l].type == THMR_LIGHT_POINT,
+               "render_meshes: light %d has type %d", l, d->lights[l].type);
+  THMR_CHECK(d->bg_layout == THMR_BG_NONE || d->bg_layout == THMR_BG_HWC || d->bg_layout == THMR_BG_CHW_NORMALIZED,
+             "render_meshes: bg_layout %d", d->bg_layout);
+  THMR_CHECK(d->bg_layout == THMR_BG_NONE || d->bg_image, "render_meshes: bg_layout set but bg_image is null");
+  THMR_CHECK(!d->composite || d->bg_layout != THMR_BG_NONE, "render_meshes: a composite needs a background image");
+  THMR_CHECK((reinterpret_cast<uintptr_t>(d->rgba) & 15) == 0, "render_meshes: rgba %p is not 16-byte aligned",
+             static_cast<void*>(d->rgba));   // written as one float4 per pixel
+  THMR_CHECK(d->n_images <= 65535, "render_meshes: n_images %d (<= 65535)", d->n_images);
+  RenderParams p;
+  memset(&p, 0, sizeof(p));
+  for (int m = 0; m < d->n_meshes; ++m) {
+    const int img = d->mesh_image_host ? d->mesh_image_host[m] : m;
+    THMR_CHECK(img >= 0 && img < d->n_images, "render_meshes: mesh %d goes to image %d, outside [0, %d)", m, img,
+               d->n_images);
+    p.mesh_image[m] = static_cast<uint16_t>(img);
+  }
+  p.verts = d->vertices; p.trans = d->translations;
+  p.faces = t->faces; p.vf_off = t->vf_off; p.vf_face = t->vf_face;
+  p.n = d->n_meshes; p.V = t->V; p.F = t->F; p.W = d->width; p.H = d->height; p.n_images = d->n_images;
+  memcpy(p.R, d->rotation, sizeof(p.R));
+  p.rotate_translation = d->rotate_translation != 0;
+  p.focal = d->focal; p.cx = 0.5f * d->width; p.cy = 0.5f * d->height; p.znear = d->znear;
+  for (int c = 0; c < 3; ++c) {
+    p.base[c] = d->base_color[c]; p.bg[c] = d->bg_color[c]; p.mean[c] = d->mean[c]; p.std[c] = d->std[c];
+  }
+  p.ambient = d->ambient;
+  p.n_lights = d->n_lights;
+  for (int l = 0; l < d->n_lights; ++l)
+    p.lights[l] = RenderLight{d->lights[l].type, d->lights[l].vec[0], d->lights[l].vec[1], d->lights[l].vec[2],
+                              d->lights[l].intensity};
+  p.bg_layout = d->bg_layout; p.bg_image = d->bg_image;
+  p.rgba = d->rgba; p.composite = d->composite; p.face_id = d->face_id; p.depth = d->depth;
+  void* ws = reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  render_carve(ws, p.V, p.n, p.n_images, p.W, p.H, &p);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long nv = static_cast<long long>(p.n) * p.V, nf = static_cast<long long>(p.n) * p.F;
+  const long long npx = static_cast<long long>(p.n_images) * p.W * p.H;
+  THMR_CUDA(cudaMemsetAsync(p.keys, 0xff, npx * sizeof(unsigned long long), st));
+  render_vertex_kernel<<<static_cast<unsigned>((nv + 255) / 256), 256, 0, st>>>(p);
+  THMR_CUDA(cudaGetLastError());
+  render_normal_kernel<<<static_cast<unsigned>((nv + 255) / 256), 256, 0, st>>>(p);
+  THMR_CUDA(cudaGetLastError());
+  render_raster_kernel<<<static_cast<unsigned>((nf + 127) / 128), 128, 0, st>>>(p);
+  THMR_CUDA(cudaGetLastError());
+  render_resolve_kernel<<<static_cast<unsigned>((npx + 255) / 256), 256, 0, st>>>(p);
+  THMR_CUDA(cudaGetLastError());
+  return THMR_OK;
 }
 
 // ------------------------------------------------------------------------------------------ SMPL
