@@ -277,6 +277,42 @@ size_t thmr_render_workspace_bytes(const thmr_render_topology* t, int n_meshes, 
  * misaligned rgba. */
 int thmr_render_meshes(const thmr_render_desc* desc, void* workspace, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Prediction grid: the reference's MeshRenderer.visualize_tensorboard / visualize
+ * [tokenhmr/lib/utils/mesh_renderer.py:57-107], with the OpenPose skeleton overlays of render_openpose.py drawn bit
+ * for bit as OpenCV 4.x draws them (DESIGN.md §2 "Rendering").  Per sample, in order: the crop, the front mesh tile,
+ * the side mesh tile, then one skeleton tile per keypoint set present (predictions, then GT), laid out as
+ * torchvision.utils.make_grid(tiles, nrow, padding, pad_value = 0) lays them out.
+ * ---------------------------------------------------------------------------------------------- */
+#define THMR_POSE_KEYPOINTS 44          /* 25 OpenPose body joints + 19 extra joints */
+#define THMR_POSE_MAX_WIDTH 11718       /* widest crop whose overlay thicknesses are line 2 / circle radius 1 */
+
+typedef struct thmr_pose_grid_desc {
+  int n;                          /* samples, 1 .. 65535 */
+  int width, height;              /* crop size, width 1 .. THMR_POSE_MAX_WIDTH, height 1 .. 16384 */
+  const float* images;            /* [n, 3, H, W] crops in [0, 1] (img * std + mean) */
+  const float* front;             /* [n, H, W, 3] front mesh tile (thmr_render_meshes composite over the crop) */
+  const float* side;              /* [n, H, W, 4] side mesh tile (thmr_render_meshes rgba; rgb is used) */
+  const float* pred_keypoints;    /* [n, 44, 2] normalised predictions (pred_keypoints_2d), or NULL */
+  const float* gt_keypoints;      /* [n, 44, 3] normalised GT with confidence (keypoints_2d), or NULL */
+  float img_res;                  /* keypoints are drawn at img_res * (kp + 0.5) (cfg.MODEL.IMAGE_SIZE) */
+  int nrow;                       /* grid columns requested, >= 1 */
+  int padding;                    /* 0 .. 1024 */
+  float* out;                     /* [3, grid_h, grid_w] with unit column stride; see thmr_pose_grid_size */
+  int64_t out_stride_c, out_stride_y;   /* elements; out_stride_y >= grid_w, out_stride_c >= grid_h * out_stride_y */
+} thmr_pose_grid_desc;
+
+/* The grid's size in pixels for these sizes (pure arithmetic); THMR_ERR_INVALID for sizes out of range. */
+int thmr_pose_grid_size(int n, int width, int height, int n_keypoint_sets, int nrow, int padding, int* grid_h,
+                        int* grid_w);
+/* Workspace of one thmr_pose_grid call (pure arithmetic; 0 for sizes out of range). */
+size_t thmr_pose_grid_workspace_bytes(int n, int width, int height, int n_keypoint_sets);
+/* Writes the whole grid.  Stream-ordered, no host synchronisation, no allocation: CUDA-graph capturable.  Returns
+ * THMR_ERR_INVALID, with nothing launched, for a null desc / images / front / side / out / workspace, sizes or
+ * strides out of range, or a non-finite img_res.  A keypoint whose pixel coordinate lies outside int32 (where the
+ * reference's cv2 call raises) is not drawn. */
+int thmr_pose_grid(const thmr_pose_grid_desc* desc, void* workspace, void* stream);
+
 /* ================================================================================================
  * Engine: TokenHMR.forward(batch)  [tokenhmr.py:330-338 -> 135-188]
  * ============================================================================================== */

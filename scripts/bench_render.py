@@ -1,9 +1,12 @@
-"""Times the CUDA rasterizer (tokenhmr_b200.render): render_crops of 64 crops at 256 x 256, and 1920 x 1080 frames with
-1, 8 and 32 people, on a closed synthetic mesh of SMPL's size (6890 vertices, 13776 faces).  CUDA events around
+"""Times the CUDA rasterizer (tokenhmr_b200.render): render_crops of 64 crops at 256 x 256, 1920 x 1080 frames with
+1, 8 and 32 people, and MeshRenderer.visualize_tensorboard (eval.py --render's prediction grid: two mesh views and two
+OpenPose skeletons per crop) at B = 8 (what eval.py renders) and 64, on a closed synthetic mesh of SMPL's size (6890
+vertices, 13776 faces).  CUDA events around
 windows of back-to-back calls of at least --window-ms each, --repeats times after --warmup calls; prints one JSON line
 with the median, the spread (max - min over median) and the card's name and power limit read in the same run.
 
-There is no CPU or pyrender baseline: pyrender needs an OpenGL stack this project does not depend on."""
+There is no CPU or pyrender baseline: pyrender needs an OpenGL stack this project does not depend on, and the
+reference's render_openpose no longer runs on NumPy >= 1.24 (np.int)."""
 from __future__ import annotations
 
 import argparse
@@ -83,6 +86,20 @@ def main():
         r = _time(fn, a.warmup, a.window_ms, a.repeats)
         res[f"frame_1080p_{n}"] = dict(r, tris_per_s=n * faces.shape[0] / r["ms"] * 1e3,
                                        pix_per_s=1920 * 1080 / r["ms"] * 1e3)
+    mr = R.MeshRenderer({"EXTRA": {"FOCAL_LENGTH": 5000.0}, "MODEL": {"IMAGE_SIZE": 256}}, faces, "cuda:0")
+    for B in (8, 64):
+        v = torch.from_numpy(posed(v0, B, seed=B)).cuda()
+        t = torch.tensor(np.stack([rng.uniform(-.1, .1, B), rng.uniform(-.1, .1, B),
+                                   2 * 5000. / (256 * rng.uniform(.6, 1., B))], 1), dtype=torch.float32, device="cuda")
+        imgs = torch.rand(B, 3, 256, 256, device="cuda")
+        pred = torch.rand(B, 44, 2, device="cuda") - 0.5
+        gt = torch.cat([torch.rand(B, 44, 2, device="cuda") - 0.5, (torch.rand(B, 44, 1, device="cuda") > 0.3).float()],
+                       -1)
+        r = _time(lambda: mr.visualize_tensorboard(v, t, imgs, pred, gt), a.warmup, a.window_ms, a.repeats)
+        res[f"visualize_tensorboard_{B}x256"] = dict(r, what="CUDA-tensor inputs, grid left on the GPU")
+        args = [x.cpu().numpy() for x in (v, t, imgs, pred, gt)]
+        r = _time(lambda: mr.visualize_tensorboard(*args).cpu().numpy(), a.warmup, a.window_ms, a.repeats)
+        res[f"visualize_tensorboard_{B}x256_numpy"] = dict(r, what="numpy inputs and .cpu().numpy(), as eval.py calls it")
     print(json.dumps(res))
 
 

@@ -112,6 +112,17 @@ class RenderDesc(Structure):
                 ("rgba", c_void_p), ("composite", c_void_p), ("face_id", c_void_p), ("depth", c_void_p)]
 
 
+POSE_KEYPOINTS = 44
+POSE_MAX_WIDTH = 11718
+
+
+class PoseGridDesc(Structure):
+    _fields_ = [("n", c_int), ("width", c_int), ("height", c_int), ("images", c_void_p), ("front", c_void_p),
+                ("side", c_void_p), ("pred_keypoints", c_void_p), ("gt_keypoints", c_void_p), ("img_res", c_float),
+                ("nrow", c_int), ("padding", c_int), ("out", c_void_p), ("out_stride_c", c_int64),
+                ("out_stride_y", c_int64)]
+
+
 class Outputs(Structure):
     _fields_ = [(n, c_void_p) for n in ("cls_logits_softmax", "pred_cam", "rotmats", "betas", "pred_cam_t",
                                         "focal_length", "pred_keypoints_3d", "pred_vertices", "pred_keypoints_2d",
@@ -170,6 +181,9 @@ SIGNATURES = {
     "thmr_render_topology_destroy": (None, [c_void_p]),
     "thmr_render_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
     "thmr_render_meshes": (c_int, [POINTER(RenderDesc), c_void_p, c_void_p]),
+    "thmr_pose_grid_size": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]),
+    "thmr_pose_grid_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "thmr_pose_grid": (c_int, [POINTER(PoseGridDesc), c_void_p, c_void_p]),
     "thmr_smpl_create": (c_int, [POINTER(SmplDesc), POINTER(c_void_p)]),
     "thmr_smpl_destroy": (None, [c_void_p]),
     "thmr_smpl_workspace_bytes": (c_size_t, [c_void_p, c_int]),

@@ -8,6 +8,7 @@
 #include "engine.cuh"
 #include "engine_strict.cuh"
 #include "eval_kernels.cuh"
+#include "keypoints.cuh"
 #include "preproc.cuh"
 #include "render.cuh"
 #include "tok_encoder.cuh"
@@ -548,6 +549,73 @@ int thmr_render_meshes(const thmr_render_desc* d, void* workspace, void* stream)
   render_raster_kernel<<<static_cast<unsigned>((nf + 127) / 128), 128, 0, st>>>(p);
   THMR_CUDA(cudaGetLastError());
   render_resolve_kernel<<<static_cast<unsigned>((npx + 255) / 256), 256, 0, st>>>(p);
+  THMR_CUDA(cudaGetLastError());
+  return THMR_OK;
+}
+
+// ------------------------------------------------------------------------------------------ prediction grid
+static bool pose_grid_sizes_ok(int n, int W, int H, int sets, int nrow, int padding) {
+  return n >= 1 && n <= 65535 && W >= 1 && W <= THMR_POSE_MAX_WIDTH && H >= 1 && H <= 16384 && sets >= 0 &&
+         sets <= 2 && nrow >= 1 && padding >= 0 && padding <= 1024 &&
+         static_cast<long long>(n) * (sets > 0 ? sets : 1) * W * H <= (1ll << 32);
+}
+
+int thmr_pose_grid_size(int n, int W, int H, int sets, int nrow, int padding, int* grid_h, int* grid_w) {
+  THMR_CHECK(grid_h && grid_w, "pose_grid_size: null output");
+  THMR_CHECK(pose_grid_sizes_ok(n, W, H, sets, nrow, padding),
+             "pose_grid_size: n=%d %dx%d, %d keypoint sets, nrow=%d, padding=%d", n, W, H, sets, nrow, padding);
+  const long long tiles = static_cast<long long>(n) * (3 + sets);
+  const long long xmaps = nrow < tiles ? nrow : tiles, ymaps = (tiles + xmaps - 1) / xmaps;
+  const long long gh = ymaps * (H + padding) + padding, gw = xmaps * (W + padding) + padding;
+  THMR_CHECK(gh < (1ll << 31) && gw < (1ll << 31) && gh * gw <= (1ll << 34), "pose_grid_size: grid %lldx%lld", gw, gh);
+  *grid_h = static_cast<int>(gh);
+  *grid_w = static_cast<int>(gw);
+  return THMR_OK;
+}
+
+size_t thmr_pose_grid_workspace_bytes(int n, int W, int H, int sets) {
+  if (!pose_grid_sizes_ok(n, W, H, sets, 1, 0)) return 0;
+  return pose_grid_carve(nullptr, n, sets, W, H, nullptr) + 1024;
+}
+
+int thmr_pose_grid(const thmr_pose_grid_desc* d, void* workspace, void* stream) {
+  THMR_CHECK(d && workspace, "pose_grid: null desc or workspace");
+  THMR_CHECK(d->images && d->front && d->side && d->out, "pose_grid: null images, front, side or out");
+  const int sets = (d->pred_keypoints ? 1 : 0) + (d->gt_keypoints ? 1 : 0);
+  int gh = 0, gw = 0;
+  const int s = thmr_pose_grid_size(d->n, d->width, d->height, sets, d->nrow, d->padding, &gh, &gw);
+  if (s != THMR_OK) return s;
+  THMR_CHECK(isfinite(d->img_res), "pose_grid: img_res %g", d->img_res);
+  THMR_CHECK(d->out_stride_y >= gw && d->out_stride_c >= static_cast<int64_t>(gh) * d->out_stride_y,
+             "pose_grid: strides (%lld, %lld) do not hold a %dx%d grid", static_cast<long long>(d->out_stride_c),
+             static_cast<long long>(d->out_stride_y), gw, gh);
+  PoseGridParams p;
+  memset(&p, 0, sizeof(p));
+  p.n = d->n; p.H = d->height; p.W = d->width;
+  p.images = d->images; p.front = d->front; p.side = d->side;
+  p.kp[0] = d->pred_keypoints; p.kp[1] = d->gt_keypoints;
+  p.n_sets = 0;
+  for (int k = 0; k < 2; ++k)
+    if (p.kp[k]) p.set_of[p.n_sets++] = k;
+  p.img_res = d->img_res;
+  p.tiles = 3 + sets;
+  const long long tiles = static_cast<long long>(p.n) * p.tiles;
+  p.xmaps = static_cast<int>(d->nrow < tiles ? d->nrow : tiles);
+  p.padding = d->padding;
+  p.grid_h = gh; p.grid_w = gw;
+  p.out = d->out; p.out_sc = d->out_stride_c; p.out_sy = d->out_stride_y;
+  void* ws = reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  pose_grid_carve(ws, p.n, sets, p.W, p.H, &p);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (sets > 0) {
+    const long long npx = static_cast<long long>(p.n) * sets * p.W * p.H;
+    THMR_CUDA(cudaMemsetAsync(p.keys, 0, npx * sizeof(uint32_t), st));
+    const long long nprim = static_cast<long long>(p.n) * sets * kPosePrims;
+    pose_raster_kernel<<<static_cast<unsigned>((nprim + 127) / 128), 128, 0, st>>>(p);
+    THMR_CUDA(cudaGetLastError());
+  }
+  const long long ng = static_cast<long long>(gh) * gw;
+  pose_grid_kernel<<<static_cast<unsigned>((ng + 255) / 256), 256, 0, st>>>(p);
   THMR_CUDA(cudaGetLastError());
   return THMR_OK;
 }

@@ -275,3 +275,125 @@ class Renderer:
         res = self.raster(v, t, W, H, focal, rotation=R, rotate_translation=True, mesh_image=[0] * v.shape[0],
                           n_images=1, lights=multiple_lights(), base_color=mesh_base_color, bg_color=scene_bg_color)
         return res["rgba"][0].cpu().numpy()
+
+
+def _cuda_f32(x, dev: torch.device, name: str, shape_tail: Sequence[Optional[int]]) -> torch.Tensor:
+    """numpy array or tensor -> contiguous float32 tensor on dev, with its trailing dimensions checked."""
+    t = torch.as_tensor(np.asarray(x) if not torch.is_tensor(x) else x)
+    if t.dim() != len(shape_tail) or any(w is not None and s != w for s, w in zip(t.shape, shape_tail)):
+        want = ", ".join("*" if w is None else str(w) for w in shape_tail)
+        raise ThmrError(f"{name} must be ({want}), got {tuple(t.shape)}")
+    return t.to(dev, torch.float32).contiguous()
+
+
+class MeshRenderer:
+    """Drop-in for the reference's `MeshRenderer(cfg, faces)` (tokenhmr/lib/utils/mesh_renderer.py:44-157), the
+    renderer eval.py --render uses.  `visualize_tensorboard` returns the reference's grid -- per sample the crop, the
+    front mesh view, the side mesh view and the OpenPose skeletons of the predicted and GT keypoints -- as a CUDA
+    float32 (3, H', W') tensor, so eval.py's `.cpu().numpy()` keeps working.  The mesh tiles come from
+    `Renderer.raster`; the skeletons and the grid from `thmr_pose_grid` (csrc/keypoints.cuh), which draws them bit
+    for bit as the reference's render_openpose draws them with OpenCV.  Inputs may be numpy arrays (what eval.py
+    passes) or CUDA tensors (then nothing waits for the host); they are taken as float32, eval.py's dtype.
+
+    Reference behaviour kept on purpose (DESIGN.md §2 "Rendering"):
+      * the focal length is always cfg.EXTRA.FOCAL_LENGTH; visualize*'s `focal_length` argument is ignored (:82);
+      * `__call__` flips camera_translation[0] in place (:118), so visualize*'s side view gets the row its front view
+        already flipped and flips it back: the side view is rendered as if pred_cam_t had x negated.  This class
+        renders that side view without touching the caller's arrays;
+      * predicted keypoints get a confidence of img_res * 1.5 (the ones column is scaled too, :76-77) and always
+        take the 14 extra-joint substitutions; GT keypoints take one only where the extra joint's confidence is > 0
+        and the body joint's == 0 (:84-96).
+    Unlike the reference, no argument is modified (the reference scales gt_keypoints in place)."""
+
+    def __init__(self, cfg, faces=None, device: str | torch.device = "cuda:0"):
+        if faces is None:
+            raise ThmrError("MeshRenderer needs the mesh faces")
+        self.cfg = cfg
+        self.focal_length = float(_cfg_get(cfg, "EXTRA.FOCAL_LENGTH", getattr(cfg, "focal_length", 5000.0)))
+        self.img_res = int(_cfg_get(cfg, "MODEL.IMAGE_SIZE", getattr(cfg, "image_size", 256)))
+        self.camera_center = [self.img_res // 2, self.img_res // 2]
+        # the mesh tiles composite over the already un-normalised crop: mean 0 and std 1 make img * std + mean exact
+        self.renderer = Renderer({"EXTRA": {"FOCAL_LENGTH": self.focal_length},
+                                  "MODEL": {"IMAGE_SIZE": self.img_res, "IMAGE_MEAN": [0.0, 0.0, 0.0],
+                                            "IMAGE_STD": [1.0, 1.0, 1.0]}}, faces, device)
+        self.faces = self.renderer.faces
+        self.device = self.renderer.device
+
+    # ---------------------------------------------------------------------------------------------- mesh tiles
+    def _front(self, v, t, imgs, focal, base, ws=None):
+        """(B, H, W, 3): the mesh over the crop, color * (alpha > 0.8) + (1 - mask) * crop (:146-151)."""
+        H, W = imgs.shape[2:]
+        return self.renderer.raster(v, t, W, H, focal, lights=crop_lights(), base_color=base, bg_image=imgs,
+                                    bg_layout=_lib.BG_CHW_NORMALIZED, outputs=("composite",),
+                                    workspace=ws)["composite"]
+
+    def _side(self, v, t, H, W, focal, base, rot_angle=90.0, ws=None):
+        """(B, H, W, 4): the mesh turned rot_angle degrees about y over white; rgb is the tile."""
+        Ry = rotation_matrix(np.radians(rot_angle), [0, 1, 0])
+        return self.renderer.raster(v, t, W, H, focal, rotation=Ry, lights=crop_lights(), base_color=base,
+                                    bg_color=(1.0, 1.0, 1.0), outputs=("rgba",), workspace=ws)["rgba"]
+
+    def __call__(self, vertices, camera_translation, image, focal_length=5000, text=None, resize=None,
+                 side_view=False, baseColorFactor=(1.0, 1.0, 0.9, 1.0), rot_angle=90) -> np.ndarray:
+        """MeshRenderer.__call__ (:109-157): vertices (V, 3), camera_translation (3,) (pred_cam_t), image (H, W, 3)
+        in [0, 1]; returns (H, W, 3) float32.  `text` is unused, as in the reference; `resize` is not supported.
+        Unlike the reference, camera_translation is not flipped in place, so every call renders it unflipped."""
+        if resize is not None:
+            raise ThmrError("MeshRenderer.__call__: resize is not supported")
+        dev = self.device
+        v = _cuda_f32(vertices, dev, "vertices", (self.renderer.num_verts, 3))[None]
+        t = _cuda_f32(camera_translation, dev, "camera_translation", (3,))[None]
+        img = _cuda_f32(image, dev, "image", (None, None, 3))
+        H, W = img.shape[:2]
+        base = tuple(float(c) for c in baseColorFactor[:3])
+        if side_view:
+            out = self._side(v, t, H, W, float(focal_length), base, float(rot_angle))[0, ..., :3]
+        else:
+            out = self._front(v, t, img.permute(2, 0, 1)[None].contiguous(), float(focal_length), base)[0]
+        return out.cpu().numpy()
+
+    # ---------------------------------------------------------------------------------------------- grids
+    def visualize(self, vertices, camera_translation, images, focal_length=None, nrow=3, padding=2) -> torch.Tensor:
+        """MeshRenderer.visualize (:57-68): per sample the crop, the front and the side view."""
+        return self._grid(vertices, camera_translation, images, None, None, int(nrow), int(padding))
+
+    def visualize_tensorboard(self, vertices, camera_translation, images, pred_keypoints, gt_keypoints,
+                              focal_length=None, nrow=5, padding=2) -> torch.Tensor:
+        """MeshRenderer.visualize_tensorboard (:70-107): vertices (B, V, 3), camera_translation (B, 3) (pred_cam_t),
+        images (B, 3, H, W) crops in [0, 1], pred_keypoints (B, 44, 2) normalised or None, gt_keypoints (B, 44, 3) or
+        None.  Returns the make_grid(nrow, padding) grid, (3, B (H + 2) + 2, 5 (W + 2) + 2) with both keypoint sets
+        and the default nrow, padding."""
+        nrow = int(nrow) - (gt_keypoints is None) - (pred_keypoints is None)
+        return self._grid(vertices, camera_translation, images, pred_keypoints, gt_keypoints, nrow, int(padding))
+
+    def _grid(self, vertices, camera_translation, images, pred_keypoints, gt_keypoints, nrow: int,
+              padding: int) -> torch.Tensor:
+        dev = self.device
+        imgs = _cuda_f32(images, dev, "images", (None, 3, None, None))
+        B, _, H, W = imgs.shape
+        v = _cuda_f32(vertices, dev, "vertices", (B, self.renderer.num_verts, 3))
+        t = _cuda_f32(camera_translation, dev, "camera_translation", (B, 3))
+        kp = [None if k is None else _cuda_f32(k, dev, name, (B, _lib.POSE_KEYPOINTS, d))
+              for k, name, d in ((pred_keypoints, "pred_keypoints", 2), (gt_keypoints, "gt_keypoints", 3))]
+        n_sets = sum(k is not None for k in kp)
+        gh, gw = ctypes.c_int(), ctypes.c_int()
+        check(lib().thmr_pose_grid_size(B, W, H, n_sets, nrow, padding, ctypes.byref(gh), ctypes.byref(gw)))
+        with torch.cuda.device(dev):
+            base = (1.0, 1.0, 0.9)
+            front = self._front(v, t, imgs, self.focal_length, base)
+            # the double x flip of :118 (front view flips the row in place, the side view flips it back)
+            t_side = t.clone()
+            t_side[:, 0].neg_()
+            side = self._side(v, t_side, H, W, self.focal_length, base)
+            out = torch.empty(3, gh.value, gw.value, dtype=torch.float32, device=dev)
+            ws = torch.empty(lib().thmr_pose_grid_workspace_bytes(B, W, H, n_sets), dtype=torch.uint8, device=dev)
+            d = _lib.PoseGridDesc()
+            d.n, d.width, d.height = B, W, H
+            d.images, d.front, d.side = imgs.data_ptr(), front.data_ptr(), side.data_ptr()
+            d.pred_keypoints = kp[0].data_ptr() if kp[0] is not None else None
+            d.gt_keypoints = kp[1].data_ptr() if kp[1] is not None else None
+            d.img_res = float(self.img_res)
+            d.nrow, d.padding = nrow, padding
+            d.out, d.out_stride_c, d.out_stride_y = out.data_ptr(), out.stride(0), out.stride(1)
+            check(lib().thmr_pose_grid(ctypes.byref(d), ws.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        return out
