@@ -36,6 +36,24 @@ struct Step {
   const char* name;
   double flops;   // algorithmic FLOPs (2*MAC) of tensor-core work, 0 for bandwidth-bound kernels
   double bytes;   // algorithmic HBM bytes for bandwidth-bound kernels, 0 otherwise
+  int kernels;    // kernels fn launches (memcpys are not kernels): thmr_engine_num_launches is their sum
+};
+
+constexpr int kMaxStamps = 2048;
+
+// A mode's step list while it is built: tag() sets the label and work of the steps pushed after it, slot() is the
+// in-graph start stamp slot of the next step (nullptr when the mode records no stamps or the slots are used up).
+struct StepList {
+  std::vector<Step>& v;
+  unsigned long long* stamps;   // [kMaxStamps] or nullptr
+  const char* name = "";
+  double flops = 0, bytes = 0;
+  void tag(const char* n, double f = 0, double b = 0) { name = n; flops = f; bytes = b; }
+  void push_back(StepFn fn, int kernels = 1) { v.push_back(Step{std::move(fn), name, flops, bytes, kernels}); }
+  size_t size() const { return v.size(); }
+  unsigned long long* slot() const {
+    return stamps && v.size() < static_cast<size_t>(kMaxStamps - 1) ? stamps + v.size() : nullptr;
+  }
 };
 
 // ---- SMPL stage (shared by thmr_lbs / thmr_smpl_forward / the engine) -----------------------------------
@@ -126,15 +144,65 @@ struct thmr_engine {
   int B = 0;
   std::vector<thmr::Step> steps;
   size_t vit_steps = 0;  // steps [0, vit_steps) = backbone
-  int launches = 0;      // kernels per forward (strict mode counts them while building; 0 = default-path formula)
   unsigned long long* stamps = nullptr;   // [kMaxStamps] in the workspace: start stamp of step i, end stamp at [n_steps]
 };
-
-constexpr int kMaxStamps = 2048;
 
 namespace thmr {
 
 constexpr int kTokPad = 3;  // zero rows on both ends of every tokenizer-decoder sequence (max dilation)
+
+// The forward's last step, the same in every mode: read-out assembly, 6D -> rotation (token_head.py:103-128), SMPL +
+// projection (tokenhmr.py:162-187).  carve() takes the buffers that stand in for the outputs a caller leaves null and
+// the SMPL workspace; push() plans the blend GEMM of every kSmplChunk-pose chunk and appends the step.
+struct SmplTail {
+  float *rot, *betas, *cam, *camt, *focal, *kp3, *kp2, *verts;
+  SmplWs ws;
+
+  void carve(Bump& bp, const SmplModel& m, int B) {
+    rot = bp.take<float>(static_cast<size_t>(B) * 24 * 9);
+    betas = bp.take<float>(static_cast<size_t>(B) * 16);
+    cam = bp.take<float>(static_cast<size_t>(B) * 4);
+    camt = bp.take<float>(static_cast<size_t>(B) * 4);
+    focal = bp.take<float>(static_cast<size_t>(B) * 2);
+    const int NJ = 25 + m.n_extra;
+    kp3 = bp.take<float>(static_cast<size_t>(B) * NJ * 3);
+    kp2 = bp.take<float>(static_cast<size_t>(B) * NJ * 2);
+    verts = bp.take<float>(static_cast<size_t>(B) * m.V * 3);
+    smpl_carve(bp, m, B, &ws);
+  }
+
+  // readout: [B, 32] read-out GEMM output; out6: [B, Lpj, 8] 6D rotations with kTokPad pad rows either side
+  int push(StepList& S, const thmr_engine* e, int B, const float* readout, const float* out6, int Lpj) const {
+    const thmr_smpl* sm = e->smpl;
+    int err = THMR_OK;
+    std::vector<GemmPlan> blend((B + kSmplChunk - 1) / kSmplChunk);
+    for (int ci = 0, p0 = 0; p0 < B; p0 += kSmplChunk, ++ci) {
+      const int s = smpl_blend_plan(sm->m, ws, p0, (B - p0) < kSmplChunk ? (B - p0) : kSmplChunk, &blend[ci]);
+      if (s != THMR_OK) err = s;
+    }
+    const float* ip = e->w.init_pose; const float* ib = e->w.init_betas; const float* ic = e->w.init_cam;
+    const int nb = sm->m.nb;
+    const float focal_length = e->cfg.focal_length, isz = static_cast<float>(e->cfg.image_size);
+    const SmplTail fb = *this;
+    S.tag("smpl.lbs");
+    S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
+      float* rot = r.out.rotmats ? r.out.rotmats : fb.rot;
+      float* bet = r.out.betas ? r.out.betas : fb.betas;
+      float* cam = r.out.pred_cam ? r.out.pred_cam : fb.cam;
+      head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(readout, 32, out6, 8, Lpj, kTokPad, ip, ib, ic, rot,
+                                                                bet, cam, r.out.pose6d, B, nb);
+      THMR_CUDA(cudaGetLastError());
+      float* verts = r.out.pred_vertices ? r.out.pred_vertices : fb.verts;
+      float* kp3 = r.out.pred_keypoints_3d ? r.out.pred_keypoints_3d : fb.kp3;
+      float* kp2 = r.out.pred_keypoints_2d ? r.out.pred_keypoints_2d : fb.kp2;
+      float* camt = r.out.pred_cam_t ? r.out.pred_cam_t : fb.camt;
+      float* foc = r.out.focal_length ? r.out.focal_length : fb.focal;
+      return smpl_run(sm, rot, 0, bet, B, verts, nullptr, kp3, cam, focal_length, isz, camt, foc, kp2, fb.ws,
+                      blend.data(), st);
+    }, 3 + 2 * static_cast<int>(blend.size()));   // assemble, pose, joints; blend GEMM + skinning per chunk (smpl_run)
+    return err;
+  }
+};
 
 inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, int* status, cudaStream_t stream) {
   const thmr_config& c = e->cfg;
@@ -187,40 +255,25 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   const int Lj = c.tok_joints, Lpj = Lj + 2 * PAD;
   float* x32 = bp.take<float>(static_cast<size_t>(B) * Lpj * W);
   float* out6 = bp.take<float>(static_cast<size_t>(B) * Lpj * 8);
-  float* rot_fb = bp.take<float>(static_cast<size_t>(B) * 24 * 9);
-  float* betas_fb = bp.take<float>(static_cast<size_t>(B) * 16);
-  float* cam_fb = bp.take<float>(static_cast<size_t>(B) * 4);
-  float* camt_fb = bp.take<float>(static_cast<size_t>(B) * 4);
-  float* focal_fb = bp.take<float>(static_cast<size_t>(B) * 2);
-  const int NJ = 25 + e->smpl->m.n_extra;
-  float* kp3_fb = bp.take<float>(static_cast<size_t>(B) * NJ * 3);
-  float* kp2_fb = bp.take<float>(static_cast<size_t>(B) * NJ * 2);
-  float* verts_fb = bp.take<float>(static_cast<size_t>(B) * e->smpl->m.V * 3);
-  SmplWs sws;
-  smpl_carve(bp, e->smpl->m, B, &sws);
+  SmplTail tail;
+  tail.carve(bp, e->smpl->m, B);
   // fp8 mode: xn and h hold e4m3 codes inside their fp16 buffers; their power-of-two scales are k-block-major
-  // [cols / 128][ld_sc], ld_sc = M + 128 so that every 128-row tile of every sub-batch reads a full 512-byte run
+  // [cols / 128][ld_sc], ld_sc = M + 128 (at least M rounded up to 128) so that every 128-row tile, the last one too,
+  // reads a full 512-byte run
   const int ld_sc = M + 128;
+  const int F = c.vit_mlp_ratio * D;
   float* xn_sc = c.fp8 ? bp.take<float>(static_cast<size_t>(D / 128) * ld_sc) : nullptr;
-  float* h_sc = c.fp8 ? bp.take<float>(static_cast<size_t>(c.vit_mlp_ratio * D / 128) * ld_sc) : nullptr;
+  float* h_sc = c.fp8 ? bp.take<float>(static_cast<size_t>(F / 128) * ld_sc) : nullptr;
   const size_t total = (bp.off + 1023) & ~size_t(1023);
   if (!build) return total;
 
   // ---------------------------------------------------------------- steps
   e->steps.clear();
-  struct StepList {
-    std::vector<Step>& v;
-    const char* name = "";
-    double flops = 0, bytes = 0;
-    void tag(const char* n, double f = 0, double b = 0) { name = n; flops = f; bytes = b; }
-    void push_back(StepFn fn) { v.push_back(Step{std::move(fn), name, flops, bytes}); }
-    size_t size() const { return v.size(); }
-  } S{e->steps};
-  int err = THMR_OK;
   e->stamps = stamps;
-  auto slot = [&]() -> unsigned long long* { return S.size() < static_cast<size_t>(kMaxStamps - 1) ? stamps + S.size() : nullptr; };
+  StepList S{e->steps, stamps};
+  int err = THMR_OK;
   auto add_gemm = [&](GemmDesc d) {
-    d.stamp = slot();
+    d.stamp = S.slot();
     GemmPlan plan;
     const int s = gemm_make_plan(d, &plan);
     if (s != THMR_OK) { err = s; return; }
@@ -238,44 +291,51 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
     d.out32 = o32; d.ld32 = N; d.out16 = o16; d.ld16 = N;
     add_gemm(d);
   };
-  // fp8 mode: A and B are e4m3 codes with their block scales; o8 (nullable) = e4m3 output + its scales
-  auto linear8 = [&](const uint8_t* A, const float* a_sc, int rows, const void* Wt, const float* w_sc, int N, int K,
-                     const float* bias, int act, float* o32, __half* o16, const float* resid, uint8_t* o8,
-                     float* o8_sc) {
-    GemmDesc d;
-    d.fp8 = 1;
-    d.A = reinterpret_cast<const __half*>(A); d.lda = K; d.a_rows = rows;
-    d.B = static_cast<const __half*>(Wt); d.ldb = K;
-    d.M = rows; d.N = N; d.K = K;
-    d.bias = bias; d.act = act; d.resid = resid; d.ldr = N;
-    d.out32 = o32; d.ld32 = N; d.out16 = o16; d.ld16 = N;
-    d.a_scale = a_sc; d.ld_as = ld_sc; d.w_scale = w_sc;
-    d.out8 = o8; d.ld8 = N; d.out8_scale = o8_sc; d.ld8s = ld_sc;
-    add_gemm(d);
-  };
-  auto ln8 = [&](const float* in, const float* g, const float* b, uint8_t* o8, float* o_sc, int R, int C, float eps) {
-    S.flops = 0;
-    S.bytes = static_cast<double>(R) * C * 5;
-    unsigned long long* sp = slot();
-    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
-      return layernorm_e4m3_launch(in, g, b, o8, o_sc, ld_sc, nullptr, R, C, eps, st, sp);
-    });
-  };
   auto ln = [&](const float* in, const float* g, const float* b, __half* o16, float* o32, int R, int C, float eps,
                 int relu, int out_t) {
     S.flops = 0;
     S.bytes = static_cast<double>(R) * C * (4 + (o16 ? 2 : 0) + (o32 ? 4 : 0));
-    unsigned long long* sp = slot();
+    unsigned long long* sp = S.slot();
     S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       return layernorm_launch(in, g, b, o16, 0, o32, R, C, eps, relu, out_t, st, sp);
     });
+  };
+  // The ViT blocks differ by mode only in these two helpers.  LayerNorm of the residual stream x into xn: fp16, or in
+  // fp8 mode e4m3 codes with their scales xn_sc.
+  auto ln_xn = [&](const float* g, const float* b) {
+    if (!c.fp8) return ln(x, g, b, xn, nullptr, M, D, c.vit_ln_eps, 0, 0);
+    S.flops = 0;
+    S.bytes = static_cast<double>(M) * D * 5;
+    uint8_t* xn8 = reinterpret_cast<uint8_t*>(xn);
+    const float eps = c.vit_ln_eps;
+    unsigned long long* sp = S.slot();
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
+      return layernorm_e4m3_launch(x, g, b, xn8, xn_sc, ld_sc, nullptr, M, D, eps, st, sp);
+    });
+  };
+  // GEMM over the M token rows reading xn or h (K columns, with their scales a_sc in fp8 mode).  fp8 mode: e4m3 A and
+  // weights (block scales w_sc) on the FP8 tensor cores, and an output with scales o_sc (fc1's h) is stored as e4m3
+  // codes in o16's buffer.
+  auto linear_xn = [&](const __half* A, const float* a_sc, int K, const void* Wt, const float* w_sc, int N,
+                       const float* bias, int act, float* o32, __half* o16, float* o_sc, const float* resid = nullptr) {
+    if (!c.fp8) return linear(A, K, M, Wt, N, K, bias, act, o32, o16, resid);
+    GemmDesc d;
+    d.fp8 = 1;
+    d.A = A; d.lda = K; d.a_rows = M;
+    d.B = static_cast<const __half*>(Wt); d.ldb = K;
+    d.M = M; d.N = N; d.K = K;
+    d.bias = bias; d.act = act; d.resid = resid; d.ldr = N;
+    d.out32 = o32; d.ld32 = N; d.out16 = o_sc ? nullptr : o16; d.ld16 = N;
+    d.a_scale = a_sc; d.ld_as = ld_sc; d.w_scale = w_sc;
+    d.out8 = o_sc ? reinterpret_cast<uint8_t*>(o16) : nullptr; d.ld8 = N; d.out8_scale = o_sc; d.ld8s = ld_sc;
+    add_gemm(d);
   };
 
   // ---- ViT backbone (vit.py:320-343)
   {
     const int S_ = c.image_size, x0 = (c.image_size - c.crop_w) / 2, Wc = c.crop_w, P = c.patch, pad = c.patch_pad;
     S.tag("vit.patch_im2col", 0, static_cast<double>(B) * 3 * c.image_size * c.crop_w * 4 + static_cast<double>(M) * KP * 2);
-    unsigned long long* sp = slot();
+    unsigned long long* sp = S.slot();
     S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
       const long total_t = static_cast<long>(B) * gh * gw * 3 * P;
       im2col_patch_kernel<<<static_cast<unsigned>((total_t + 255) / 256), 256, 0, st>>>(r.img, a0, B, S_, x0, Wc, P, pad,
@@ -292,82 +352,36 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
     d.out32 = x; d.ld32 = D;
     add_gemm(d);
   }
-  // THMR_VIT_SUB=n: run the 32 blocks over sub-batches of n images (all blocks of one sub-batch, then the next), so
-  // that a sub-batch's activations (x, xn, qkv, ao, h: 2.7 MB per image) stay resident in the 50 MB L2 between the
-  // kernel that writes them and the one that reads them; the price is smaller GEMMs (fewer tiles per wave) and the
-  // weights being streamed once per sub-batch.  0 (default) = the whole batch at once.
-  static const int env_sub = [] { const char* v = getenv("THMR_VIT_SUB"); return v ? atoi(v) : 0; }();
-  const int sub = (env_sub > 0 && env_sub < B) ? env_sub : B;
-  for (int b0 = 0; b0 < B; b0 += sub) {
-  const int bn = (B - b0) < sub ? (B - b0) : sub;
-  const int Ms = bn * T;
-  const size_t r0 = static_cast<size_t>(b0) * T;
-  float* xs = x + r0 * D;
-  __half* xns = xn + r0 * D;
-  __half* qkvs = qkv + r0 * 3 * D;
-  __half* aos = ao + r0 * D;
-  __half* hs = hbuf + r0 * c.vit_mlp_ratio * D;
-  for (int i = 0; i < c.vit_depth && c.fp8; ++i) {
-    // fp8 mode: LN -> e4m3 xn -> QKV (fp16 qkv), attention and proj as by default, LN -> e4m3 xn -> fc1 + GELU ->
-    // e4m3 h -> fc2 into the fp32 residual stream
+  for (int i = 0; i < c.vit_depth; ++i) {
     const thmr_vit_block& bw = e->blocks[i];
-    const thmr_vit_block_scales& bs = e->block_scales[i];
-    uint8_t* xn8 = reinterpret_cast<uint8_t*>(xns);
-    uint8_t* h8 = reinterpret_cast<uint8_t*>(hs);
-    const int F = c.vit_mlp_ratio * D;
+    const thmr_vit_block_scales bs = c.fp8 ? e->block_scales[i] : thmr_vit_block_scales{};
     S.tag("vit.layernorm");
-    ln8(xs, bw.ln1_g, bw.ln1_b, xn8, xn_sc + r0, Ms, D, c.vit_ln_eps);
+    ln_xn(bw.ln1_g, bw.ln1_b);
     S.tag("vit.qkv_gemm");
-    linear8(xn8, xn_sc + r0, Ms, bw.qkv_w, bs.qkv_ws, 3 * D, D, bw.qkv_b, kActNone, nullptr, qkvs, nullptr, nullptr,
-            nullptr);
-    {
-      S.tag("vit.attention", 4.0 * bn * H * 192.0 * 192.0 * 80.0, 4.0 * Ms * D * 2);
-      AttnPlan ap;
-      const int s = attention_make_plan(qkvs, 3 * D, bn, H, aos, D, nullptr, &ap);
-      if (s != THMR_OK) err = s;
-      ap.p.stamp = slot();
-      S.push_back([ap](const RunCtx&, cudaStream_t st) -> int { return attention_dispatch(ap, st); });
-    }
-    S.tag("vit.proj_gemm");
-    linear(aos, D, Ms, bw.proj_w, D, D, bw.proj_b, kActNone, xs, nullptr, xs);
-    S.tag("vit.layernorm");
-    ln8(xs, bw.ln2_g, bw.ln2_b, xn8, xn_sc + r0, Ms, D, c.vit_ln_eps);
-    S.tag("vit.fc1_gelu_gemm");
-    linear8(xn8, xn_sc + r0, Ms, bw.fc1_w, bs.fc1_ws, F, D, bw.fc1_b, kActGelu, nullptr, nullptr, nullptr, h8,
-            h_sc + r0);
-    S.tag("vit.fc2_gemm");
-    linear8(h8, h_sc + r0, Ms, bw.fc2_w, bs.fc2_ws, D, F, bw.fc2_b, kActNone, xs, nullptr, xs, nullptr, nullptr);
-  }
-  for (int i = 0; i < c.vit_depth && !c.fp8; ++i) {
-    const thmr_vit_block& bw = e->blocks[i];
-    S.tag("vit.layernorm");
-    ln(xs, bw.ln1_g, bw.ln1_b, xns, nullptr, Ms, D, c.vit_ln_eps, 0, 0);
-    S.tag("vit.qkv_gemm");
-    linear(xns, D, Ms, bw.qkv_w, 3 * D, D, bw.qkv_b, kActNone, nullptr, qkvs);
+    linear_xn(xn, xn_sc, D, bw.qkv_w, bs.qkv_ws, 3 * D, bw.qkv_b, kActNone, nullptr, qkv, nullptr);
     {
       // 4*N*N*d FLOPs per head (QK^T + PV); Q,K,V read + O written once in fp16
-      S.tag("vit.attention", 4.0 * bn * H * 192.0 * 192.0 * 80.0, 4.0 * Ms * D * 2);
+      S.tag("vit.attention", 4.0 * B * H * 192.0 * 192.0 * 80.0, 4.0 * M * D * 2);
       AttnPlan ap;
-      const int s = attention_make_plan(qkvs, 3 * D, bn, H, aos, D, nullptr, &ap);
+      const int s = attention_make_plan(qkv, 3 * D, B, H, ao, D, nullptr, &ap);
       if (s != THMR_OK) err = s;
-      ap.p.stamp = slot();
+      ap.p.stamp = S.slot();
       S.push_back([ap](const RunCtx&, cudaStream_t st) -> int { return attention_dispatch(ap, st); });
     }
     S.tag("vit.proj_gemm");
-    linear(aos, D, Ms, bw.proj_w, D, D, bw.proj_b, kActNone, xs, nullptr, xs);
+    linear(ao, D, M, bw.proj_w, D, D, bw.proj_b, kActNone, x, nullptr, x);
     S.tag("vit.layernorm");
-    ln(xs, bw.ln2_g, bw.ln2_b, xns, nullptr, Ms, D, c.vit_ln_eps, 0, 0);
+    ln_xn(bw.ln2_g, bw.ln2_b);
     S.tag("vit.fc1_gelu_gemm");
-    linear(xns, D, Ms, bw.fc1_w, c.vit_mlp_ratio * D, D, bw.fc1_b, kActGelu, nullptr, hs);
+    linear_xn(xn, xn_sc, D, bw.fc1_w, bs.fc1_ws, F, bw.fc1_b, kActGelu, nullptr, hbuf, h_sc);
     S.tag("vit.fc2_gemm");
-    linear(hs, c.vit_mlp_ratio * D, Ms, bw.fc2_w, D, c.vit_mlp_ratio * D, bw.fc2_b, kActNone, xs, nullptr, xs);
-  }
+    linear_xn(hbuf, h_sc, F, bw.fc2_w, bs.fc2_ws, D, bw.fc2_b, kActNone, x, nullptr, nullptr, x);
   }
   {
     S.tag("vit.layernorm", 0, static_cast<double>(M) * D * 6);
     const float* g = w.last_g; const float* b = w.last_b;
     const float eps = c.vit_ln_eps;
-    unsigned long long* sp = slot();
+    unsigned long long* sp = S.slot();
     S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
       float* t32 = r.vit_tokens_only ? r.vit_tokens_only : r.out.vit_tokens;
       return layernorm_launch(x, g, b, feat, 0, t32, M, D, eps, 0, 0, st, sp);
@@ -499,33 +513,7 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   conv(bufA, Lcur, W, w.conv_post, W, 1, 3, kActNone, 0, nullptr, 0, bufB, nullptr);
   conv(bufB, Lcur, W, w.conv_out, 6, 1, 3, kActNone, 0, out6, 8, nullptr, nullptr);
 
-  S.tag("smpl.lbs");
-  // ---- read-out assembly, 6D -> rotation (token_head.py:103-128), SMPL + projection (tokenhmr.py:162-187)
-  {
-    const float* ip = w.init_pose; const float* ib = w.init_betas; const float* ic = w.init_cam;
-    const int nb = e->smpl->m.nb;
-    const thmr_smpl* sm = e->smpl;
-    std::vector<GemmPlan> blend((B + kSmplChunk - 1) / kSmplChunk);
-    for (int ci = 0, p0 = 0; p0 < B; p0 += kSmplChunk, ++ci) {
-      const int s = smpl_blend_plan(sm->m, sws, p0, (B - p0) < kSmplChunk ? (B - p0) : kSmplChunk, &blend[ci]);
-      if (s != THMR_OK) err = s;
-    }
-    const float focal = c.focal_length, isz = static_cast<float>(c.image_size);
-    S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
-      float* rot = r.out.rotmats ? r.out.rotmats : rot_fb;
-      float* bet = r.out.betas ? r.out.betas : betas_fb;
-      float* cam = r.out.pred_cam ? r.out.pred_cam : cam_fb;
-      head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(readout, 32, out6, 8, Lpj, PAD, ip, ib, ic, rot, bet, cam,
-                                                                r.out.pose6d, B, nb);
-      THMR_CUDA(cudaGetLastError());
-      float* verts = r.out.pred_vertices ? r.out.pred_vertices : verts_fb;
-      float* kp3 = r.out.pred_keypoints_3d ? r.out.pred_keypoints_3d : kp3_fb;
-      float* kp2 = r.out.pred_keypoints_2d ? r.out.pred_keypoints_2d : kp2_fb;
-      float* camt = r.out.pred_cam_t ? r.out.pred_cam_t : camt_fb;
-      float* foc = r.out.focal_length ? r.out.focal_length : focal_fb;
-      return smpl_run(sm, rot, 0, bet, B, verts, nullptr, kp3, cam, focal, isz, camt, foc, kp2, sws, blend.data(), st);
-    });
-  }
+  if (const int s = tail.push(S, e, B, readout, out6, Lpj); s != THMR_OK) err = s;
   *status = err;
   // zero the padded fp16 probability buffer once (pad rows are never written afterwards)
   if (err == THMR_OK) {

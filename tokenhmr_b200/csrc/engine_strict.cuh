@@ -68,33 +68,16 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   float* bufA = bp.take<float>(static_cast<size_t>(B) * Lp0 * W);
   float* bufB = bp.take<float>(static_cast<size_t>(B) * Lp0 * W);
   float* out6 = bp.take<float>(static_cast<size_t>(B) * Lpj * 8);
-  float* rot_fb = bp.take<float>(static_cast<size_t>(B) * 24 * 9);
-  float* betas_fb = bp.take<float>(static_cast<size_t>(B) * 16);
-  float* cam_fb = bp.take<float>(static_cast<size_t>(B) * 4);
-  float* camt_fb = bp.take<float>(static_cast<size_t>(B) * 4);
-  float* focal_fb = bp.take<float>(static_cast<size_t>(B) * 2);
-  const int NJ = 25 + e->smpl->m.n_extra;
-  float* kp3_fb = bp.take<float>(static_cast<size_t>(B) * NJ * 3);
-  float* kp2_fb = bp.take<float>(static_cast<size_t>(B) * NJ * 2);
-  float* verts_fb = bp.take<float>(static_cast<size_t>(B) * e->smpl->m.V * 3);
-  SmplWs sws;
-  smpl_carve(bp, e->smpl->m, B, &sws);
+  SmplTail tail;
+  tail.carve(bp, e->smpl->m, B);
   const size_t total = (bp.off + 1023) & ~size_t(1023);
   if (!build) return total;
 
   // ---------------------------------------------------------------- steps
   e->steps.clear();
   e->stamps = nullptr;       // (in-graph stamps are a default-mode instrument)
-  struct StepList {
-    std::vector<Step>& v;
-    const char* name = "";
-    double flops = 0, bytes = 0;
-    void tag(const char* n, double f = 0, double b = 0) { name = n; flops = f; bytes = b; }
-    void push_back(StepFn fn) { v.push_back(Step{std::move(fn), name, flops, bytes}); }
-    size_t size() const { return v.size(); }
-  } S{e->steps};
+  StepList S{e->steps, nullptr};
   int err = THMR_OK;
-  int launches = 0;
 
   // split(A32) + GEMM over K' = 3K.  `rows` = GEMM M; (sT, spitch, slo) = optional padded-sequence remap of the split;
   // conv: taps > 1 reads A' rows shifted by tap_row0 + t * tap_stride (A' row = [hi | lo | hi] of cin channels).
@@ -126,8 +109,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       THMR_TRY(split_rows_launch(A, lda, dst, srows, K, act, sT, sp, slo, st));
       return gemm_launch(plan, st);
-    });
-    launches += 2;
+    }, 2);
   };
   auto lin = [&](const float* A, int K, long rows, int act_in, const void* Wt, int N, const float* bias, float* o32,
                  const float* resid = nullptr) {
@@ -142,15 +124,13 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       return layernorm_launch(in, g, b, nullptr, 0, o32, R, C, eps, relu, out_t, st);
     });
-    launches += 1;
   };
-  auto push1 = [&](StepFn fn) { S.push_back(std::move(fn)); launches += 1; };
 
   // ---- ViT backbone (vit.py:320-343)
   {
     const int S_ = c.image_size, x0 = (c.image_size - c.crop_w) / 2, Wc = c.crop_w, P = c.patch, pad = c.patch_pad;
     S.tag("vit.patch_im2col", 0, static_cast<double>(B) * 3 * c.image_size * c.crop_w * 4 + static_cast<double>(M) * KP * 4);
-    push1([=](const RunCtx& r, cudaStream_t st) -> int {
+    S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
       const long total_t = static_cast<long>(B) * gh * gw * 3 * P;
       im2col_patch_f32_kernel<<<static_cast<unsigned>((total_t + 255) / 256), 256, 0, st>>>(r.img, a0, B, S_, x0, Wc, P,
                                                                                            pad, gh, gw);
@@ -171,7 +151,9 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     S.tag("vit.qkv_gemm");
     lin(xn, D, M, kSplitActNone, bw.qkv_w, 3 * D, bw.qkv_b, qkv);
     S.tag("vit.attention", 4.0 * B * H * 192.0 * 192.0 * 80.0, 4.0 * M * D * 4);
-    push1([=](const RunCtx&, cudaStream_t st) -> int { return attention_f32_launch(qkv, 3 * D, B, H, ao, D, att_scale, st); });
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
+      return attention_f32_launch(qkv, 3 * D, B, H, ao, D, att_scale, st);
+    });
     S.tag("vit.proj_gemm");
     lin(ao, D, M, kSplitActNone, bw.proj_w, D, bw.proj_b, x, x);
     S.tag("vit.layernorm");
@@ -185,7 +167,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     S.tag("vit.layernorm", 0, static_cast<double>(M) * D * 8);
     const float* g = w.last_g; const float* b = w.last_b;
     const float eps = c.vit_ln_eps;
-    push1([=](const RunCtx& r, cudaStream_t st) -> int {
+    S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
       THMR_TRY(layernorm_launch(x, g, b, nullptr, 0, feat, M, D, eps, 0, 0, st));
       float* t32 = r.vit_tokens_only ? r.vit_tokens_only : r.out.vit_tokens;
       if (t32) THMR_CUDA(cudaMemcpyAsync(t32, feat, sizeof(float) * M * D, cudaMemcpyDeviceToDevice, st));
@@ -200,7 +182,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   S.tag("dec.token_ops");
   {
     const float* t0 = w.token0;
-    push1([=](const RunCtx&, cudaStream_t st) -> int {
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       broadcast_row_kernel<<<(B * E + 255) / 256, 256, 0, st>>>(t0, tok, B, E);
       THMR_CUDA(cudaGetLastError());
       return THMR_OK;
@@ -216,7 +198,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     {
       const int ld = L * 2 * inner, koff = l * 2 * inner, voff = koff + inner, heads = c.dec_heads;
       const float scale = 1.0f / sqrtf(static_cast<float>(c.dec_dim_head));
-      push1([=](const RunCtx&, cudaStream_t st) -> int {
+      S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
         dec_cross_attn_f32_kernel<192><<<B * heads, 192, 0, st>>>(q32, kv, ld, koff, voff, scale, att32, heads);
         THMR_CUDA(cudaGetLastError());
         return THMR_OK;
@@ -227,12 +209,11 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     lin(y32, E, B, kSplitActNone, dw.ff1_w, c.dec_mlp_dim, dw.ff1_b, hid32);
     lin(hid32, c.dec_mlp_dim, B, kSplitActGelu, dw.ff2_w, E, dw.ff2_b, tok, tok);
   }
-  push1([=](const RunCtx& r, cudaStream_t st) -> int {
+  S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
     if (r.out.token_out)
       THMR_CUDA(cudaMemcpyAsync(r.out.token_out, tok, sizeof(float) * B * E, cudaMemcpyDeviceToDevice, st));
     return THMR_OK;
-  });
-  launches -= 1;   // (a memcpy node, not a kernel)
+  }, 0);
   lin(tok, E, B, kSplitActNone, w.readout_w, 32, w.readout_b, readout);
 
   // ---- token classifier (token_classifier.py:89-104)
@@ -244,7 +225,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
     ln(cx, mw.ln1_g, mw.ln1_b, yT, B * TN, CH, c.ln_eps, 0, TN);                      // transposed: (B*H, T)
     lin(yT, TN, static_cast<long>(B) * CH, kSplitActNone, mw.tok1_w, c.cls_token_inter, mw.tok1_b, t1);
     lin(t1, c.cls_token_inter, static_cast<long>(B) * CH, kSplitActGelu, mw.tok2_w, TN, mw.tok2_b, yT2);
-    push1([=](const RunCtx&, cudaStream_t st) -> int {
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       const long n = static_cast<long>(B) * TN * CH;
       mixer_add_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(cx, yT2, nullptr, xy, B, TN, CH);
       THMR_CUDA(cudaGetLastError());
@@ -266,7 +247,6 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
       THMR_CUDA(cudaMemcpyAsync(probs_fallback, p32, sizeof(float) * B * TN * NC, cudaMemcpyDeviceToDevice, st));
     return THMR_OK;
   });
-  launches += 1;
 
   S.tag("tok.decoder_ops");
   // ---- tokenizer: soft codebook lookup + Conv1d decoder (vanilla_pose_vqvae.py:294-297, 135-154)
@@ -294,7 +274,8 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   conv(d32, Lcur, c.code_dim, kSplitActNone, w.conv_in, W, 1, 3, bufA, W, nullptr);
   for (int u = 0; u < c.n_upsample; ++u) {
     const int Lout = c.upsample_sizes[u], Lin = Lcur;
-    push1([=](const RunCtx&, cudaStream_t st) -> int {      // nearest gather commutes with ReLU: copy the pre-ReLU rows
+    // nearest gather commutes with ReLU: copy the pre-ReLU rows
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       const long n = static_cast<long>(B) * (Lout + 2 * PAD) * (W / 4);
       upsample_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(
           reinterpret_cast<const __half*>(bufA), reinterpret_cast<__half*>(bufB), B, Lin, Lout, PAD, W / 4);
@@ -309,7 +290,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   float* xres = bufA;
   {
     const long n4 = static_cast<long>(B) * (Lcur + 2 * PAD) * W / 4;
-    push1([=](const RunCtx&, cudaStream_t st) -> int {
+    S.push_back([=](const RunCtx&, cudaStream_t st) -> int {
       relu_inplace_kernel<<<static_cast<unsigned>((n4 + 255) / 256), 256, 0, st>>>(xres, n4);
       THMR_CUDA(cudaGetLastError());
       return THMR_OK;
@@ -324,34 +305,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   conv(xres, Lcur, W, kSplitActNone, w.conv_post, W, 1, 3, bufB, W, nullptr);
   conv(bufB, Lcur, W, kSplitActNone, w.conv_out, 6, 1, 3, out6, 8, nullptr);
 
-  S.tag("smpl.lbs");
-  {
-    const float* ip = w.init_pose; const float* ib = w.init_betas; const float* ic = w.init_cam;
-    const int nb = e->smpl->m.nb;
-    const thmr_smpl* sm = e->smpl;
-    std::vector<GemmPlan> blend((B + kSmplChunk - 1) / kSmplChunk);
-    for (int ci = 0, p0 = 0; p0 < B; p0 += kSmplChunk, ++ci) {
-      const int s = smpl_blend_plan(sm->m, sws, p0, (B - p0) < kSmplChunk ? (B - p0) : kSmplChunk, &blend[ci]);
-      if (s != THMR_OK) err = s;
-    }
-    const float focal = c.focal_length, isz = static_cast<float>(c.image_size);
-    S.push_back([=](const RunCtx& r, cudaStream_t st) -> int {
-      float* rot = r.out.rotmats ? r.out.rotmats : rot_fb;
-      float* bet = r.out.betas ? r.out.betas : betas_fb;
-      float* cam = r.out.pred_cam ? r.out.pred_cam : cam_fb;
-      head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(readout, 32, out6, 8, Lpj, PAD, ip, ib, ic, rot, bet, cam,
-                                                                r.out.pose6d, B, nb);
-      THMR_CUDA(cudaGetLastError());
-      float* verts = r.out.pred_vertices ? r.out.pred_vertices : verts_fb;
-      float* kp3 = r.out.pred_keypoints_3d ? r.out.pred_keypoints_3d : kp3_fb;
-      float* kp2 = r.out.pred_keypoints_2d ? r.out.pred_keypoints_2d : kp2_fb;
-      float* camt = r.out.pred_cam_t ? r.out.pred_cam_t : camt_fb;
-      float* foc = r.out.focal_length ? r.out.focal_length : focal_fb;
-      return smpl_run(sm, rot, 0, bet, B, verts, nullptr, kp3, cam, focal, isz, camt, foc, kp2, sws, blend.data(), st);
-    });
-    launches += 5;
-  }
-  e->launches = launches;
+  if (const int s = tail.push(S, e, B, readout, out6, Lpj); s != THMR_OK) err = s;
   *status = err;
   return total;
 }

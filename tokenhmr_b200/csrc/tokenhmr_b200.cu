@@ -797,11 +797,16 @@ int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr
 
 void thmr_engine_destroy(thmr_engine* e) { delete e; }
 
+// Runs the builder of the engine's numeric mode: returns the workspace size and, with `build`, plans the steps over it.
+static size_t engine_build_mode(thmr_engine* e, void* workspace, int B, bool build, int* status, cudaStream_t st) {
+  return e->cfg.strict ? engine_build_strict(e, workspace, B, build, status, st)
+                       : engine_build(e, workspace, B, build, status, st);
+}
+
 size_t thmr_engine_workspace_bytes(const thmr_engine* e, int max_batch) {
   if (!e || max_batch <= 0) return 0;
   int st;
-  if (e->cfg.strict) return engine_build_strict(const_cast<thmr_engine*>(e), nullptr, max_batch, false, &st, nullptr);
-  return engine_build(const_cast<thmr_engine*>(e), nullptr, max_batch, false, &st, nullptr);
+  return engine_build_mode(const_cast<thmr_engine*>(e), nullptr, max_batch, false, &st, nullptr);
 }
 
 static int engine_prepare(thmr_engine* e, int B, void* workspace, cudaStream_t st) {
@@ -810,8 +815,7 @@ static int engine_prepare(thmr_engine* e, int B, void* workspace, cudaStream_t s
   if (e->ws != workspace || e->B != B) {
     int status = THMR_OK;
     e->ws = nullptr;
-    if (e->cfg.strict) engine_build_strict(e, workspace, B, true, &status, st);
-    else engine_build(e, workspace, B, true, &status, st);
+    engine_build_mode(e, workspace, B, true, &status, st);
     if (status != THMR_OK) { e->steps.clear(); return status; }
     e->ws = workspace;
     e->B = B;
@@ -891,9 +895,9 @@ int thmr_engine_profile(thmr_engine* e, const float* img, int B, const thmr_outp
 
 int thmr_engine_num_launches(const thmr_engine* e) {
   if (!e) return 0;
-  // every step is one kernel except the SMPL tail (assemble + pose + blend GEMM + skin + joints = 5)
-  if (e->cfg.strict) return e->launches;
-  return e->steps.empty() ? 0 : static_cast<int>(e->steps.size()) + 4;
+  int n = 0;
+  for (const auto& step : e->steps) n += step.kernels;
+  return n;
 }
 
 // ------------------------------------------------------------------------------------------ multi-GPU exchange
