@@ -181,6 +181,21 @@ int thmr_smpl_forward(const thmr_smpl* m, const float* rotmats /* [B,24,3,3] */,
                       float* verts, float* joints, const float* pred_cam, float focal_length, float image_size,
                       float* cam_t, float* focal_out, float* kp2d, void* workspace, void* stream);
 
+/* Gradients of the body model (DESIGN §2 "SMPL gradients").  Stateless: each call takes the forward's inputs and
+ * the output cotangents and recomputes the forward's intermediates with its own kernels, on the caller's stream, without
+ * host synchronisation (graph-capturable).  Reductions run in a fixed order, so two calls give bitwise-equal results.
+ * The workspace is its own (thmr_smpl_backward_workspace_bytes), not the forward's. */
+size_t thmr_smpl_backward_workspace_bytes(const thmr_smpl* m, int batch);
+/* VJP of thmr_smpl_forward (without the camera tail): grad_verts [B,V,3] and grad_joints [B,25+n_extra,3]
+ * are nullable (null = zero cotangent); writes grad_rotmats [B,24,3,3] and grad_betas [B,num_betas]. */
+int thmr_smpl_backward(const thmr_smpl* m, const float* rotmats, const float* betas, int B,
+                       const float* grad_verts, const float* grad_joints,
+                       float* grad_rotmats, float* grad_betas, void* workspace, void* stream);
+/* VJP of thmr_lbs: grad_joints is over the 24 J_transformed joints; grad_pose is [B,24,3] (pose2rot) or [B,24,3,3]. */
+int thmr_lbs_backward(const thmr_smpl* m, const float* pose, int pose2rot, const float* betas, int B,
+                      const float* grad_verts, const float* grad_joints,
+                      float* grad_pose, float* grad_betas, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Tokenizer encoder + hard quantisation (SURVEY §8 row f4): EncodeTokens
  * [tokenization/models/vanilla_pose_vqvae.py:304-346 -> PoseSPEncoderV1 :42-111, quantize_cnn.py:74-86]

@@ -190,6 +190,11 @@ SIGNATURES = {
     "thmr_lbs": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "thmr_smpl_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_float,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "thmr_smpl_backward_workspace_bytes": (c_size_t, [c_void_p, c_int]),
+    "thmr_smpl_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p]),
+    "thmr_lbs_backward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),
     "thmr_engine_workspace_bytes": (c_size_t, [c_void_p, c_int]),

@@ -44,6 +44,14 @@ struct SmplModel {
   int* extra_vid = nullptr;       // [21] VertexJointSelector ids
   int* joint_map = nullptr;       // [25]
   int parents[kSmplJ];
+  // backward only (smpl_grad.cuh)
+  float* basis32 = nullptr;       // [207 + nb, off_pitch] fp32 [posedirs ; shapedirs^T], pad columns zero
+  int* bw_ptr = nullptr;          // [nvb*24 + 1] per (256-vertex block, joint): list of the block's vertices ...
+  int* bw_lv = nullptr;           // ... (local index) skinned to that joint ...
+  float* bw_val = nullptr;        // ... and their weights, vertices in increasing order
+  int* cx_ptr = nullptr;          // [V + 1] per vertex: the grad_joints rows that read it (CSC of the joint map's
+  int* cx_row = nullptr;          //         extra-vertex picks, weight 1, then of joint_regressor_extra)
+  float* cx_val = nullptr;
 };
 
 // ---- init-time: J_template / J_shapedirs (one block per output scalar) ---------------------------------

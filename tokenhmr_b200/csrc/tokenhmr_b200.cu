@@ -11,6 +11,7 @@
 #include "keypoints.cuh"
 #include "preproc.cuh"
 #include "render.cuh"
+#include "smpl_grad.cuh"
 #include "tok_encoder.cuh"
 
 using namespace thmr;
@@ -627,6 +628,8 @@ void thmr_smpl_destroy(thmr_smpl* s) {
   cudaFree(m.v_template); cudaFree(m.shapedirs); cudaFree(m.J_template); cudaFree(m.J_shapedirs);
   cudaFree(m.posedirsT); cudaFree(m.w_idx); cudaFree(m.w_val); cudaFree(m.jx_ptr); cudaFree(m.jx_idx);
   cudaFree(m.jx_val); cudaFree(m.extra_vid); cudaFree(m.joint_map); cudaFree(s->parents_dev);
+  cudaFree(m.basis32); cudaFree(m.bw_ptr); cudaFree(m.bw_lv); cudaFree(m.bw_val); cudaFree(m.cx_ptr);
+  cudaFree(m.cx_row); cudaFree(m.cx_val);
   delete s;
 }
 
@@ -669,6 +672,14 @@ int thmr_smpl_create(const thmr_smpl_desc* d, thmr_smpl** out) {
     smpl_pack_posedirs_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(pd, m.shapedirs, m.v_template, nb,
                                                                                m.posedirsT, 3 * V);
   }
+  {
+    // the backward's fp32 blend basis, rows at the offsets pitch (smpl_carve)
+    const long pitch = (3L * V + 3) / 4 * 4;
+    const long n = static_cast<long>(kSmplFeatBeta + nb) * pitch;
+    SM_TRY(dev_alloc(&m.basis32, static_cast<size_t>(n)));
+    smpl_pack_basis32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256>>>(pd, m.shapedirs, nb, m.basis32, 3 * V,
+                                                                              pitch);
+  }
   cudaError_t ce = cudaDeviceSynchronize();
   cudaFree(Jreg);
   cudaFree(pd);
@@ -696,11 +707,36 @@ int thmr_smpl_create(const thmr_smpl_desc* d, thmr_smpl** out) {
     m.ell = ell;
     SM_TRY(dev_upload(&m.w_idx, idx));
     SM_TRY(dev_upload(&m.w_val, val));
+    // backward: per (256-vertex block, joint) the block's vertices skinned to the joint, in vertex order
+    const int nvb = (V + kBwdVerts - 1) / kBwdVerts;
+    std::vector<int> bptr(1, 0), blv;
+    std::vector<float> bval;
+    for (int vb = 0; vb < nvb; ++vb)
+      for (int j = 0; j < kSmplJ; ++j) {
+        for (int v = vb * kBwdVerts; v < std::min(V, (vb + 1) * kBwdVerts); ++v)
+          for (int k = 0; k < ell; ++k)
+            if (val[static_cast<size_t>(v) * ell + k] != 0.f && idx[static_cast<size_t>(v) * ell + k] == j) {
+              blv.push_back(v - vb * kBwdVerts);
+              bval.push_back(val[static_cast<size_t>(v) * ell + k]);
+            }
+        bptr.push_back(static_cast<int>(blv.size()));
+      }
+    SM_TRY(dev_upload(&m.bw_ptr, bptr));
+    SM_TRY(dev_upload(&m.bw_lv, blv));
+    SM_TRY(dev_upload(&m.bw_val, bval));
   }
-  // extra joint regressor -> CSR
+  for (int i = 0; i < 21; ++i)
+    if (d->extra_vertex_ids_host[i] < 0 || d->extra_vertex_ids_host[i] >= V)
+      return bail(fail(THMR_ERR_INVALID, "smpl_create: extra vertex id %d out of range", d->extra_vertex_ids_host[i]));
+  // extra joint regressor -> CSR (forward) and, with the joint map's extra-vertex picks, a per-vertex CSC (backward)
   {
     std::vector<int> ptr(1, 0), idx;
     std::vector<float> val;
+    std::vector<std::vector<std::pair<int, float>>> col(V);
+    for (int k = 0; k < 25; ++k) {
+      const int src = d->joint_map_host[k];
+      if (src >= kSmplJ && src < kSmplJ + 21) col[d->extra_vertex_ids_host[src - kSmplJ]].push_back({k, 1.f});
+    }
     if (m.n_extra > 0) {
       std::vector<float> Jx(static_cast<size_t>(m.n_extra) * V);
       if (cudaMemcpy(Jx.data(), d->joint_regressor_extra, Jx.size() * sizeof(float), cudaMemcpyDefault) != cudaSuccess)
@@ -708,7 +744,7 @@ int thmr_smpl_create(const thmr_smpl_desc* d, thmr_smpl** out) {
       for (int r = 0; r < m.n_extra; ++r) {
         for (int v = 0; v < V; ++v) {
           const float w = Jx[static_cast<size_t>(r) * V + v];
-          if (w != 0.f) { idx.push_back(v); val.push_back(w); }
+          if (w != 0.f) { idx.push_back(v); val.push_back(w); col[v].push_back({25 + r, w}); }
         }
         ptr.push_back(static_cast<int>(idx.size()));
       }
@@ -716,10 +752,16 @@ int thmr_smpl_create(const thmr_smpl_desc* d, thmr_smpl** out) {
     SM_TRY(dev_upload(&m.jx_ptr, ptr));
     SM_TRY(dev_upload(&m.jx_idx, idx));
     SM_TRY(dev_upload(&m.jx_val, val));
+    std::vector<int> cptr(1, 0), crow;
+    std::vector<float> cval;
+    for (int v = 0; v < V; ++v) {
+      for (const auto& e : col[v]) { crow.push_back(e.first); cval.push_back(e.second); }
+      cptr.push_back(static_cast<int>(crow.size()));
+    }
+    SM_TRY(dev_upload(&m.cx_ptr, cptr));
+    SM_TRY(dev_upload(&m.cx_row, crow));
+    SM_TRY(dev_upload(&m.cx_val, cval));
   }
-  for (int i = 0; i < 21; ++i)
-    if (d->extra_vertex_ids_host[i] < 0 || d->extra_vertex_ids_host[i] >= V)
-      return bail(fail(THMR_ERR_INVALID, "smpl_create: extra vertex id %d out of range", d->extra_vertex_ids_host[i]));
   SM_TRY(dev_upload(&m.extra_vid, std::vector<int>(d->extra_vertex_ids_host, d->extra_vertex_ids_host + 21)));
   SM_TRY(dev_upload(&m.joint_map, std::vector<int>(d->joint_map_host, d->joint_map_host + 25)));
 #undef SM_TRY
@@ -755,6 +797,35 @@ int thmr_smpl_forward(const thmr_smpl* s, const float* rotmats, const float* bet
   smpl_carve(bp, s->m, B, &ws);
   return smpl_run(s, rotmats, 0, betas, B, verts, nullptr, joints, pred_cam, focal_length, image_size, cam_t, focal_out,
                   kp2d, ws, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+size_t thmr_smpl_backward_workspace_bytes(const thmr_smpl* s, int batch) {
+  if (!s || batch <= 0) return 0;
+  Bump bp(nullptr);
+  SmplBwdWs ws;
+  smpl_bwd_carve(bp, s->m, batch, &ws);
+  return (bp.off + 1023) & ~size_t(1023);
+}
+
+int thmr_smpl_backward(const thmr_smpl* s, const float* rotmats, const float* betas, int B, const float* grad_verts,
+                       const float* grad_joints, float* grad_rotmats, float* grad_betas, void* workspace, void* stream) {
+  THMR_CHECK(s && rotmats && betas && grad_rotmats && grad_betas && workspace && B > 0, "smpl_backward: bad argument");
+  Bump bp(workspace);
+  SmplBwdWs ws;
+  smpl_bwd_carve(bp, s->m, B, &ws);
+  return smpl_backward_run(s, rotmats, 0, betas, B, grad_verts, grad_joints, 0, grad_rotmats, grad_betas, ws,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int thmr_lbs_backward(const thmr_smpl* s, const float* pose, int pose2rot, const float* betas, int B,
+                      const float* grad_verts, const float* grad_joints, float* grad_pose, float* grad_betas,
+                      void* workspace, void* stream) {
+  THMR_CHECK(s && pose && betas && grad_pose && grad_betas && workspace && B > 0, "lbs_backward: bad argument");
+  Bump bp(workspace);
+  SmplBwdWs ws;
+  smpl_bwd_carve(bp, s->m, B, &ws);
+  return smpl_backward_run(s, pose, pose2rot ? 1 : 0, betas, B, grad_verts, grad_joints, 1, grad_pose, grad_betas, ws,
+                           static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------ engine

@@ -41,12 +41,26 @@ GATHERED_FIELDS = ("pred_vertices", "pred_keypoints_3d", "pred_keypoints_2d", "p
                    "rotmats", "betas")
 
 
+class SmplOutput(NamedTuple):
+    """The fields of the reference SMPL.forward output (smpl_wrapper.py:27-41) that its callers read."""
+    vertices: torch.Tensor   # (B, V, 3)
+    joints: torch.Tensor     # (B, 25 + n_extra, 3): 25 OpenPose joints + the regressed extra joints
+
+
 class _SmplFacade:
-    """`model.smpl.faces` is read by demo.py:52."""
+    """`model.smpl`: `.faces` is read by demo.py:52; `model.smpl(global_orient=, body_pose=, betas=)` is the reference
+    SMPL wrapper's forward on rotation matrices, differentiable in all three (SMPLifyInv, tokenhmr_b200.fitting)."""
 
     def __init__(self, model: SMPLModel):
         self._model = model
         self.faces = model.faces
+
+    def __call__(self, global_orient: torch.Tensor, body_pose: torch.Tensor, betas: torch.Tensor,
+                 pose2rot: bool = False) -> SmplOutput:
+        """global_orient (B,1,3,3), body_pose (B,23,3,3), betas (B,nb), CUDA fp32.  pose2rot is ignored, as the
+        reference's SMPLLayer ignores it (tokenhmr.py:176): the inputs are always rotation matrices."""
+        verts, joints = self._model.forward(global_orient, body_pose, betas)
+        return SmplOutput(verts, joints)
 
 
 class TokenHMREngine(nn.Module):

@@ -210,6 +210,7 @@ class SMPLModel:
         torch.cuda.synchronize(device)
         self.handle = h
         self._ws: Optional[torch.Tensor] = None
+        self._bws: Optional[torch.Tensor] = None
         self.faces = smpl.get("faces")
 
     def __del__(self):
@@ -226,8 +227,20 @@ class SMPLModel:
             self._ws = torch.empty(need, device=self.device, dtype=torch.uint8)
         return self._ws
 
+    def backward_workspace(self, batch: int) -> torch.Tensor:
+        need = lib().thmr_smpl_backward_workspace_bytes(self.handle, batch)
+        if self._bws is None or self._bws.numel() < need:
+            self._bws = torch.empty(need, device=self.device, dtype=torch.uint8)
+        return self._bws
+
     def lbs(self, betas: torch.Tensor, pose: torch.Tensor, pose2rot: bool = True):
-        """smplx.lbs.lbs: returns (verts (B,V,3), J_transformed (B,24,3))."""
+        """smplx.lbs.lbs: returns (verts (B,V,3), J_transformed (B,24,3)).  Differentiable in pose and betas when grad
+        mode is on and one of them requires grad (thmr_lbs_backward)."""
+        if _wants_grad(betas, pose):
+            return _LbsFn.apply(self, betas, pose, bool(pose2rot))
+        return self._lbs(betas, pose, pose2rot)
+
+    def _lbs(self, betas: torch.Tensor, pose: torch.Tensor, pose2rot: bool):
         betas, pose = _req(betas, torch.float32, "betas"), _req(pose, torch.float32, "pose")
         B = betas.shape[0]
         verts = torch.empty(B, self.num_verts, 3, device=self.device)
@@ -239,7 +252,20 @@ class SMPLModel:
     def forward(self, global_orient: torch.Tensor, body_pose: torch.Tensor, betas: torch.Tensor,
                 pred_cam: Optional[torch.Tensor] = None, focal_length: float = 5000.0, image_size: float = 256.0):
         """tokenhmr SMPL wrapper forward (smpl_wrapper.py:27-41): rotation matrices -> (vertices, 44 joints)
-        [+ (cam_t, focal, keypoints_2d) when pred_cam is given: tokenhmr.py:165-187]."""
+        [+ (cam_t, focal, keypoints_2d) when pred_cam is given: tokenhmr.py:165-187].  Without pred_cam it is
+        differentiable in global_orient, body_pose and betas when grad mode is on and one of them requires grad
+        (thmr_smpl_backward); the camera tail has no backward, so pred_cam with such inputs raises."""
+        if _wants_grad(global_orient, body_pose, betas):
+            if pred_cam is not None:
+                raise _lib.ThmrError("SMPLModel.forward: the camera tail (pred_cam) has no backward; call it without "
+                                     "pred_cam and project in PyTorch, or run it under torch.no_grad()")
+            B = betas.shape[0]
+            rot = torch.cat([global_orient.reshape(B, -1, 3, 3), body_pose.reshape(B, -1, 3, 3)], 1)
+            return _SmplForwardFn.apply(self, rot, betas)
+        return self._forward(global_orient, body_pose, betas, pred_cam, focal_length, image_size)
+
+    def _forward(self, global_orient: torch.Tensor, body_pose: torch.Tensor, betas: torch.Tensor,
+                 pred_cam: Optional[torch.Tensor] = None, focal_length: float = 5000.0, image_size: float = 256.0):
         B = betas.shape[0]
         rot = torch.cat([global_orient.reshape(B, -1, 3, 3), body_pose.reshape(B, -1, 3, 3)], 1)
         rot, betas = _req(rot, torch.float32, "rotmats"), _req(betas, torch.float32, "betas")
@@ -256,3 +282,78 @@ class SMPLModel:
                                       joints.data_ptr(), _ptr(pred_cam), focal_length, image_size, _ptr(cam_t),
                                       _ptr(focal), _ptr(kp2d), self.workspace(B).data_ptr(), _stream()))
         return (verts, joints) if pred_cam is None else (verts, joints, cam_t, focal, kp2d)
+
+    def smpl_backward(self, rotmats: torch.Tensor, betas: torch.Tensor, grad_verts: Optional[torch.Tensor],
+                      grad_joints: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """thmr_smpl_backward: rotmats (B,24,3,3), betas (B,nb), cotangents of (vertices, joints) (None = zero) ->
+        (grad_rotmats (B,24,3,3), grad_betas (B,nb))."""
+        rotmats, betas = _req(rotmats, torch.float32, "rotmats"), _req(betas, torch.float32, "betas")
+        B = betas.shape[0]
+        gv = None if grad_verts is None else _req(grad_verts, torch.float32, "grad_verts")
+        gj = None if grad_joints is None else _req(grad_joints, torch.float32, "grad_joints")
+        g_rot = torch.empty(B, 24, 3, 3, device=self.device)
+        g_betas = torch.empty(B, self.num_betas, device=self.device)
+        check(lib().thmr_smpl_backward(self.handle, rotmats.data_ptr(), betas.data_ptr(), B, _ptr(gv), _ptr(gj),
+                                       g_rot.data_ptr(), g_betas.data_ptr(), self.backward_workspace(B).data_ptr(),
+                                       _stream()))
+        return g_rot, g_betas
+
+    def lbs_backward(self, betas: torch.Tensor, pose: torch.Tensor, pose2rot: bool, grad_verts: Optional[torch.Tensor],
+                     grad_joints: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """thmr_lbs_backward: cotangents of (verts, J_transformed) (None = zero) -> (grad_pose shaped as pose,
+        grad_betas (B,nb))."""
+        betas, pose = _req(betas, torch.float32, "betas"), _req(pose, torch.float32, "pose")
+        B = betas.shape[0]
+        gv = None if grad_verts is None else _req(grad_verts, torch.float32, "grad_verts")
+        gj = None if grad_joints is None else _req(grad_joints, torch.float32, "grad_joints")
+        g_pose = torch.empty(B, 24, 3, device=self.device) if pose2rot else torch.empty(B, 24, 3, 3, device=self.device)
+        g_betas = torch.empty(B, self.num_betas, device=self.device)
+        check(lib().thmr_lbs_backward(self.handle, pose.data_ptr(), int(pose2rot), betas.data_ptr(), B, _ptr(gv),
+                                      _ptr(gj), g_pose.data_ptr(), g_betas.data_ptr(),
+                                      self.backward_workspace(B).data_ptr(), _stream()))
+        return g_pose.view(pose.shape), g_betas
+
+
+def _wants_grad(*ts: torch.Tensor) -> bool:
+    return torch.is_grad_enabled() and any(t.requires_grad for t in ts)
+
+
+class _SmplForwardFn(torch.autograd.Function):
+    """SMPLModel.forward without the camera tail, with thmr_smpl_backward as its backward."""
+
+    @staticmethod
+    def forward(ctx, model: SMPLModel, rot: torch.Tensor, betas: torch.Tensor):
+        ctx.set_materialize_grads(False)
+        ctx.model = model
+        ctx.save_for_backward(rot, betas)
+        return model._forward(rot[:, :1], rot[:, 1:], betas)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_verts, grad_joints):
+        rot, betas = ctx.saved_tensors
+        if grad_verts is None and grad_joints is None:
+            return None, None, None
+        g_rot, g_betas = ctx.model.smpl_backward(rot.reshape(rot.shape[0], 24, 3, 3), betas, grad_verts, grad_joints)
+        return (None, g_rot.view(rot.shape) if ctx.needs_input_grad[1] else None,
+                g_betas if ctx.needs_input_grad[2] else None)
+
+
+class _LbsFn(torch.autograd.Function):
+    """SMPLModel.lbs with thmr_lbs_backward as its backward."""
+
+    @staticmethod
+    def forward(ctx, model: SMPLModel, betas: torch.Tensor, pose: torch.Tensor, pose2rot: bool):
+        ctx.set_materialize_grads(False)
+        ctx.model, ctx.pose2rot = model, pose2rot
+        ctx.save_for_backward(betas, pose)
+        return model._lbs(betas, pose, pose2rot)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_verts, grad_joints):
+        betas, pose = ctx.saved_tensors
+        if grad_verts is None and grad_joints is None:
+            return None, None, None, None
+        g_pose, g_betas = ctx.model.lbs_backward(betas, pose, ctx.pose2rot, grad_verts, grad_joints)
+        return (None, g_betas if ctx.needs_input_grad[1] else None, g_pose if ctx.needs_input_grad[2] else None, None)
