@@ -196,6 +196,36 @@ int thmr_lbs_backward(const thmr_smpl* m, const float* pose, int pose2rot, const
                       const float* grad_verts, const float* grad_joints,
                       float* grad_pose, float* grad_betas, void* workspace, void* stream);
 
+/* SMPLify-inverse [tokenhmr/lib/utils/smplify_invert.py:32-156] as one stream-ordered call (DESIGN §2 "Fused
+ * SMPLify-inverse"): per iteration the body model's forward, the loss and its cotangents, the stop test, the body
+ * model's backward and torch.optim.Adam's step (lr step_size, betas (0.9, 0.999), eps 1e-8) on global_orient, body_pose
+ * and pred_cam_t, all on the device; then the final forward.  No host synchronisation and no allocation inside the call
+ * (graph-capturable); bitwise reproducible.  The loop stops before the step at the first iteration where
+ * loss < loss_thresh_f3d and fit2D < loss_thresh_f2d (compared in double); later iterations change nothing.
+ * All pointers are device pointers, fp32 unless noted; J = num_joints must equal 25 + n_extra. */
+typedef struct thmr_smplify_desc {
+  int B;                          /* >= 1 */
+  int num_iters;                  /* >= 0 */
+  int num_joints;                 /* J */
+  double step_size, margin, loss_thresh_f2d, loss_thresh_f3d;
+  float* global_orient;           /* [B,1,3,3] in/out (rotation matrices) */
+  float* body_pose;               /* [B,23,3,3] in/out */
+  float* pred_cam_t;              /* [B,3] in/out */
+  const float* betas;             /* [B,num_betas] (not optimised) */
+  const float* focal_length;      /* [B,2] */
+  const float* gt_keypoints_2d;   /* [B,J,3]; the confidence column is read but unused, as in the reference */
+  const float* gt_keypoints_3d;   /* [B,J,3] */
+  float* vertices;                /* [B,V,3]  final forward */
+  float* joints;                  /* [B,J,3]  final forward */
+  float* pj2ds;                   /* [B,J,2]  joints projected at focal_length / 256 */
+  float* reprojection_loss;       /* [1]      camera_fitting_loss of the final forward */
+  float* history;                 /* [num_iters,3] (loss, fit2D, mean push3D) per iteration run, zero after (may be
+                                     NULL when num_iters == 0) */
+  int32_t* iters_run;             /* [1]      iterations run (history rows written) */
+} thmr_smplify_desc;
+size_t thmr_smplify_workspace_bytes(const thmr_smpl* m, int B, int num_iters);
+int thmr_smplify_inv(const thmr_smpl* m, const thmr_smplify_desc* desc, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Tokenizer encoder + hard quantisation (SURVEY §8 row f4): EncodeTokens
  * [tokenization/models/vanilla_pose_vqvae.py:304-346 -> PoseSPEncoderV1 :42-111, quantize_cnn.py:74-86]

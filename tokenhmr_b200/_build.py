@@ -1,7 +1,8 @@
 """Builds libtokenhmr_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU), and next to the test suite
 the kernel probes tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers),
-tests/libthmr_fp8_probe.so (tests/csrc/fp8_probe.cu: the same for the FP8 mode's kernels) and
-tests/libthmr_pose_probe.so (tests/csrc/pose_probe.cu: the skeleton overlay's span generator, run on the host)."""
+tests/libthmr_fp8_probe.so (tests/csrc/fp8_probe.cu: the same for the FP8 mode's kernels),
+tests/libthmr_pose_probe.so (tests/csrc/pose_probe.cu: the skeleton overlay's span generator, run on the host) and
+tests/libthmr_smplify_probe.so (tests/csrc/smplify_probe.cu: the fused SMPLify-inverse's loss and Adam kernels)."""
 from __future__ import annotations
 
 import hashlib
@@ -23,6 +24,9 @@ FP8_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_fp8_probe.stamp"
 POSE_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "pose_probe.cu"
 POSE_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_pose_probe.so"
 POSE_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_pose_probe.stamp"
+SMPLIFY_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "smplify_probe.cu"
+SMPLIFY_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_smplify_probe.so"
+SMPLIFY_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_smplify_probe.stamp"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -73,13 +77,16 @@ def _compile(src: Path, out: Path, stamp: Path, flags: list, want: str, force: b
 
 def build_probe(force: bool = False, verbose: bool = False) -> Path:
     """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so, tests/csrc/fp8_probe.cu ->
-    tests/libthmr_fp8_probe.so and tests/csrc/pose_probe.cu -> tests/libthmr_pose_probe.so (no-op when sources are
-    unchanged)."""
+    tests/libthmr_fp8_probe.so, tests/csrc/pose_probe.cu -> tests/libthmr_pose_probe.so and tests/csrc/smplify_probe.cu
+    -> tests/libthmr_smplify_probe.so (no-op when sources are unchanged)."""
     want = source_hash(probe=True)
     if FP8_PROBE_SRC.exists():
         _compile(FP8_PROBE_SRC, FP8_PROBE_PATH, FP8_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
     if POSE_PROBE_SRC.exists():
         _compile(POSE_PROBE_SRC, POSE_PROBE_PATH, POSE_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
+    if SMPLIFY_PROBE_SRC.exists():
+        _compile(SMPLIFY_PROBE_SRC, SMPLIFY_PROBE_PATH, SMPLIFY_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force,
+                 verbose)
     return _compile(PROBE_SRC, PROBE_PATH, PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
 
 

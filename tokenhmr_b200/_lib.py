@@ -24,6 +24,16 @@ class SmplDesc(Structure):
                 ("extra_vertex_ids_host", POINTER(c_int32)), ("joint_map_host", POINTER(c_int32))]
 
 
+class SmplifyDesc(Structure):
+    _fields_ = [("B", c_int), ("num_iters", c_int), ("num_joints", c_int),
+                ("step_size", ctypes.c_double), ("margin", ctypes.c_double), ("loss_thresh_f2d", ctypes.c_double),
+                ("loss_thresh_f3d", ctypes.c_double),
+                ("global_orient", c_void_p), ("body_pose", c_void_p), ("pred_cam_t", c_void_p), ("betas", c_void_p),
+                ("focal_length", c_void_p), ("gt_keypoints_2d", c_void_p), ("gt_keypoints_3d", c_void_p),
+                ("vertices", c_void_p), ("joints", c_void_p), ("pj2ds", c_void_p), ("reprojection_loss", c_void_p),
+                ("history", c_void_p), ("iters_run", c_void_p)]
+
+
 class Config(Structure):
     _fields_ = [("image_size", c_int), ("crop_w", c_int), ("patch", c_int), ("patch_pad", c_int),
                 ("vit_dim", c_int), ("vit_depth", c_int), ("vit_heads", c_int), ("vit_mlp_ratio", c_int),
@@ -195,6 +205,8 @@ SIGNATURES = {
                                    c_void_p, c_void_p]),
     "thmr_lbs_backward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p]),
+    "thmr_smplify_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int]),
+    "thmr_smplify_inv": (c_int, [c_void_p, POINTER(SmplifyDesc), c_void_p, c_void_p]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),
     "thmr_engine_workspace_bytes": (c_size_t, [c_void_p, c_int]),

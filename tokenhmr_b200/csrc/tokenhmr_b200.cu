@@ -12,6 +12,7 @@
 #include "preproc.cuh"
 #include "render.cuh"
 #include "smpl_grad.cuh"
+#include "smplify.cuh"
 #include "tok_encoder.cuh"
 
 using namespace thmr;
@@ -826,6 +827,32 @@ int thmr_lbs_backward(const thmr_smpl* s, const float* pose, int pose2rot, const
   smpl_bwd_carve(bp, s->m, B, &ws);
   return smpl_backward_run(s, pose, pose2rot ? 1 : 0, betas, B, grad_verts, grad_joints, 1, grad_pose, grad_betas, ws,
                            static_cast<cudaStream_t>(stream));
+}
+
+size_t thmr_smplify_workspace_bytes(const thmr_smpl* s, int B, int num_iters) {
+  if (!s || B <= 0 || num_iters < 0) return 0;
+  Bump bp(nullptr);
+  SmplifyWs ws;
+  smplify_carve(bp, s->m, B, num_iters, &ws);
+  return (bp.off + 1023) & ~size_t(1023);
+}
+
+int thmr_smplify_inv(const thmr_smpl* s, const thmr_smplify_desc* d, void* workspace, void* stream) {
+  THMR_CHECK(s && d && workspace, "smplify_inv: null argument");
+  THMR_CHECK(d->B >= 1, "smplify_inv: B=%d", d->B);
+  THMR_CHECK(d->num_iters >= 0, "smplify_inv: num_iters=%d", d->num_iters);
+  THMR_CHECK(d->num_joints == 25 + s->m.n_extra, "smplify_inv: %d joints, the body model has %d", d->num_joints,
+             25 + s->m.n_extra);
+  THMR_CHECK(d->global_orient && d->body_pose && d->pred_cam_t && d->betas && d->focal_length && d->gt_keypoints_2d &&
+                 d->gt_keypoints_3d,
+             "smplify_inv: missing input");
+  THMR_CHECK(d->vertices && d->joints && d->pj2ds && d->reprojection_loss && d->iters_run &&
+                 (d->history || d->num_iters == 0),
+             "smplify_inv: missing output");
+  Bump bp(workspace);
+  SmplifyWs ws;
+  smplify_carve(bp, s->m, d->B, d->num_iters, &ws);
+  return smplify_run(s, *d, ws, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------ engine
