@@ -1,24 +1,32 @@
 // Test-only probe library (tests/libthmr_probe.so): thin extern "C" wrappers around the launchers of
 // tokenhmr_b200/csrc that the engine dispatches but the product ABI does not expose (GEMM epilogue options, the
 // split-precision operand builder, the strict-mode fp32 kernels, the head and tokenizer glue kernels, every LayerNorm
-// dispatch variant, the SMPL stage's kernels).  Each wrapper launches exactly what the engine launches, with the engine's
-// grid shapes, so that tests/test_gpu_kernels.py, tests/test_gpu_strict_kernels.py and tests/test_gpu_smpl_kernels.py can
-// compare one stage at a time against fp64.
-// The product never loads this library.
+// dispatch variant, the SMPL stage's kernels, the FP8 mode's block-scaled e4m3 GEMM and e4m3 LayerNorm, and the fused
+// SMPLify-inverse's loss and Adam kernels), plus the OpenPose overlay's span generator run on the host.  Each wrapper
+// launches exactly what the engine launches, with the engine's grid shapes, so that tests/test_gpu_kernels.py,
+// tests/test_gpu_strict_kernels.py, tests/test_gpu_smpl_kernels.py, tests/test_gpu_fp8.py and
+// tests/test_gpu_smplify_fused.py can compare one stage at a time against fp64, and
+// tests/test_mesh_renderer_oracle.py can hold the span generator against live cv2 without a GPU.
+// ctypes twin: tests/probe.py.  The product never loads this library.
+#include <stdint.h>
+
 #include "../../tokenhmr_b200/csrc/attention_mma.cuh"
 #include "../../tokenhmr_b200/csrc/common.cuh"
 #include "../../tokenhmr_b200/csrc/elementwise.cuh"
 #include "../../tokenhmr_b200/csrc/engine.cuh"
 #include "../../tokenhmr_b200/csrc/gemm_host.cuh"
 #include "../../tokenhmr_b200/csrc/head_kernels.cuh"
+#include "../../tokenhmr_b200/csrc/keypoints.cuh"
 #include "../../tokenhmr_b200/csrc/smpl_lbs.cuh"
+#include "../../tokenhmr_b200/csrc/smplify.cuh"
 #include "../../tokenhmr_b200/csrc/strict.cuh"
 
 using namespace thmr;
 
 #define PROBE_API extern "C" __attribute__((visibility("default")))
 
-// Mirrors the GemmDesc fields the engine sets for a plain (non-arg-min) GEMM; ctypes twin in tests/probe.py.
+// Mirrors the GemmDesc fields the engine sets for a plain (non-arg-min) GEMM, fp16 or, with fp8 set, block-scaled e4m3
+// (A, B e4m3 codes; the block scales and the e4m3 output as GemmDesc documents them); ctypes twin in tests/probe.py.
 struct probe_gemm_desc {
   const void* A; int lda; long long a_rows;
   const void* B; int ldb;
@@ -32,6 +40,10 @@ struct probe_gemm_desc {
   int seq_pitch, seq_lo, seq_hi;
   float alpha;
   int force_bn;
+  int fp8;
+  const float* a_scale; int ld_as;
+  const float* w_scale;
+  void* out8; int ld8; float* out8_scale; int ld8s;
 };
 
 static cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
@@ -71,6 +83,9 @@ PROBE_API int probe_gemm(const probe_gemm_desc* g, void* stream) {
   d.seq_pitch = g->seq_pitch; d.seq_lo = g->seq_lo; d.seq_hi = g->seq_hi;
   d.alpha = g->alpha;
   d.force_bn = g->force_bn;
+  d.fp8 = g->fp8;
+  d.a_scale = g->a_scale; d.ld_as = g->ld_as; d.w_scale = g->w_scale;
+  d.out8 = static_cast<uint8_t*>(g->out8); d.ld8 = g->ld8; d.out8_scale = g->out8_scale; d.ld8s = g->ld8s;
   GemmPlan plan;
   THMR_TRY(gemm_make_plan(d, &plan));
   return gemm_launch(plan, as_stream(stream));
@@ -85,6 +100,11 @@ PROBE_API int probe_layernorm(const float* x, const float* gamma, const float* b
                               int R, int C, float eps, int relu, int out_t, void* stream) {
   return layernorm_launch(x, gamma, beta, static_cast<__half*>(y16), ld16, y32, R, C, eps, relu, out_t,
                           as_stream(stream));
+}
+
+PROBE_API int probe_layernorm_e4m3(const float* x, const float* gamma, const float* beta, void* y8, float* ys, int lds,
+                                   float* y32, int R, int C, float eps, void* stream) {
+  return layernorm_e4m3_launch(x, gamma, beta, static_cast<uint8_t*>(y8), ys, lds, y32, R, C, eps, as_stream(stream));
 }
 
 PROBE_API int probe_softmax_rows(const float* logits, float* p32, void* p16, int R, int C, int T, int pitch, int lo,
@@ -239,4 +259,46 @@ PROBE_API int probe_smpl_joints(const float* Jposed, const float* verts, long ve
                                                       jx_val, n_extra, joints, pred_cam, focal, image_size, cam_t,
                                                       focal_out, kp2d);
   PROBE_LAUNCHED();
+}
+
+// ---- fused SMPLify-inverse (smplify.cuh; launched by thmr_smplify_inv) ----------------------------------------------
+// smplify_loss_kernel as an iteration launches it (grad_joints / grad_cam non-null) or as the final forward does
+// (both null, pj2d non-null); no done flag
+PROBE_API int probe_smplify_loss(const float* joints, const float* cam, const float* focal, const float* kp2d,
+                                 const float* kp3d, int J, int B, float* grad_joints, float* grad_cam, float* part,
+                                 float* pj2d, void* stream) {
+  return smplify_loss_launch(joints, cam, focal, kp2d, kp3d, J, B, grad_joints, grad_cam, part, pj2d, nullptr,
+                             as_stream(stream));
+}
+
+// smplify_adam_kernel for Adam step `step` (1-based) at learning rate lr over n flat elements; no done flag
+PROBE_API int probe_smplify_adam(float* p, float* m, float* v, const float* g, long n, int step, double lr,
+                                 void* stream) {
+  return smplify_adam_launch(p, m, v, g, n, step, lr, nullptr, as_stream(stream));
+}
+
+// ---- OpenPose overlay span generator (keypoints.cuh), run on the host ----------------------------------------------
+namespace {
+struct MaskEmit {
+  uint8_t* mask;
+  int W;
+  void operator()(int y, int x0, int x1) const {
+    for (int x = x0; x <= x1; ++x) mask[static_cast<long long>(y) * W + x] = 1;
+  }
+};
+}  // namespace
+
+// kind 0: cv2.line(p0, p1, thickness 2);  kind 1 / 2: cv2.circle(p0, radius 1, thickness kind).  Sets mask[y * W + x]
+// (uint8 [H, W], caller-zeroed) to 1 on every pixel painted.  Returns 0, or -1 for a bad kind or size.
+PROBE_API int probe_pose_draw(int kind, long long x0, long long y0, long long x1, long long y1, int W, int H,
+                              uint8_t* mask) {
+  if (!mask || W < 1 || H < 1) return -1;
+  MaskEmit emit{mask, W};
+  if (kind == 0)
+    cv_line(W, H, x0, y0, x1, y1, emit);
+  else if (kind == 1 || kind == 2)
+    cv_circle(W, H, x0, y0, kind, emit);
+  else
+    return -1;
+  return 0;
 }

@@ -1,9 +1,9 @@
-"""ctypes binding of the test-only kernel probe tests/libthmr_probe.so (tests/csrc/kernel_probe.cu), plus thin
+"""ctypes binding of the test-only probe library tests/libthmr_probe.so (tests/csrc/kernel_probe.cu), plus thin
 torch-facing helpers.  Every wrapper returns a THMR status; `call` raises on a non-zero one."""
 from __future__ import annotations
 
 import ctypes
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_long, c_longlong, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_long, c_longlong, c_void_p
 from pathlib import Path
 
 PROBE_PATH = Path(__file__).resolve().parent / "libthmr_probe.so"
@@ -11,7 +11,7 @@ _probe = None
 
 
 class GemmDesc(Structure):
-    """Mirror of probe_gemm_desc (kernel_probe.cu), i.e. of the engine's GemmDesc for a plain GEMM."""
+    """Mirror of probe_gemm_desc (kernel_probe.cu), i.e. of the engine's GemmDesc for a plain fp16 or FP8 GEMM."""
     _fields_ = [("A", c_void_p), ("lda", c_int), ("a_rows", c_longlong),
                 ("B", c_void_p), ("ldb", c_int),
                 ("M", c_int), ("N", c_int), ("K", c_int),
@@ -23,10 +23,14 @@ class GemmDesc(Structure):
                 ("taps", c_int), ("cin", c_int), ("tap_row0", c_int), ("tap_stride", c_int),
                 ("seq_pitch", c_int), ("seq_lo", c_int), ("seq_hi", c_int),
                 ("alpha", c_float),
-                ("force_bn", c_int)]
+                ("force_bn", c_int),
+                ("fp8", c_int),
+                ("a_scale", c_void_p), ("ld_as", c_int),
+                ("w_scale", c_void_p),
+                ("out8", c_void_p), ("ld8", c_int), ("out8_scale", c_void_p), ("ld8s", c_int)]
 
 
-P, I, L, F = c_void_p, c_int, c_long, c_float
+P, I, L, LL, F, D = c_void_p, c_int, c_long, c_longlong, c_float, c_double
 SIGNATURES = {
     "probe_last_error": (c_char_p, []),
     "probe_gemm_desc_size": (ctypes.c_size_t, []),
@@ -34,6 +38,7 @@ SIGNATURES = {
     "probe_gemm": (c_int, [POINTER(GemmDesc), P]),
     "probe_split_rows": (c_int, [P, L, P, L, I, I, I, I, I, P]),
     "probe_layernorm": (c_int, [P, P, P, P, I, P, I, I, F, I, I, P]),
+    "probe_layernorm_e4m3": (c_int, [P, P, P, P, P, I, P, I, I, F, P]),
     "probe_softmax_rows": (c_int, [P, P, P, I, I, I, I, I, P]),
     "probe_vit_attention": (c_int, [P, I, I, P, P]),
     "probe_attention_f32": (c_int, [P, I, I, I, P, I, F, P]),
@@ -52,6 +57,9 @@ SIGNATURES = {
     "probe_smpl_blend": (c_int, [P, P, I, I, I, P, P]),
     "probe_smpl_skin": (c_int, [I, I, P, P, I, P, P, L, P, L, I, I, P]),
     "probe_smpl_joints": (c_int, [P, P, L, P, P, P, P, P, I, P, P, F, F, P, P, P, I, P]),
+    "probe_smplify_loss": (c_int, [P, P, P, P, P, I, I, P, P, P, P, P]),
+    "probe_smplify_adam": (c_int, [P, P, P, P, L, I, D, P]),
+    "probe_pose_draw": (c_int, [I, LL, LL, LL, LL, I, I, P]),
 }
 
 ACT = {"none": 0, "gelu": 1, "relu": 2}      # kActNone / kActGelu / kActRelu == kSplitAct*
@@ -103,6 +111,21 @@ def gemm(A, B, M: int, N: int, K: int, *, lda: int | None = None, ldb: int | Non
     call("probe_gemm", ctypes.byref(d), stream())
 
 
+def gemm_fp8(A8, a_scale, B8, w_scale, M: int, N: int, K: int, *, a_rows: int | None = None, bias=None, resid=None,
+             ldr: int = 0, act: str = "none", out32=None, ld32: int = 0, out16=None, ld16: int = 0, out8=None,
+             out8_scale=None, alpha: float = 1.0, force_bn: int = 0) -> None:
+    """FP8 GEMM: A8 [M, K] / B8 [N, K] e4m3 codes (float8_e4m3fn or uint8), a_scale [K/128, >= M padded to 128],
+    w_scale [ceil(N/128), K/128]; out8 (e4m3 [M, N]) with out8_scale [N/128, >= M]."""
+    # fields left out are zero; taps stays 1, the only value gemm_make_plan_fp8 accepts
+    d = GemmDesc(A=ptr(A8), lda=A8.stride(0), a_rows=a_rows if a_rows is not None else M, B=ptr(B8), ldb=B8.stride(0),
+                 M=M, N=N, K=K, bias=ptr(bias), resid=ptr(resid), ldr=ldr, act=ACT[act],
+                 out32=ptr(out32), ld32=ld32, out16=ptr(out16), ld16=ld16, taps=1, alpha=alpha, force_bn=force_bn,
+                 fp8=1, a_scale=ptr(a_scale), ld_as=a_scale.stride(0), w_scale=ptr(w_scale),
+                 out8=ptr(out8), ld8=out8.stride(0) if out8 is not None else 0,
+                 out8_scale=ptr(out8_scale), ld8s=out8_scale.stride(0) if out8_scale is not None else 0)
+    call("probe_gemm", ctypes.byref(d), stream())
+
+
 def split_rows(src, R: int, C: int, act: str = "none", T: int = 0, pitch: int = 0, lo: int = 0, dst=None,
                dst_rows: int | None = None):
     """fp32 [R, C] -> fp16 [rows, 3C] = [hi | lo | hi] of act(x) * 2^4 (strict.cuh split_rows_kernel)."""
@@ -111,6 +134,17 @@ def split_rows(src, R: int, C: int, act: str = "none", T: int = 0, pitch: int = 
         dst = torch.zeros(dst_rows if dst_rows is not None else R, 3 * C, dtype=torch.float16, device=src.device)
     call("probe_split_rows", src.data_ptr(), src.stride(0), dst.data_ptr(), R, C, ACT[act], T, pitch, lo, stream())
     return dst
+
+
+def layernorm_e4m3(x, gamma, beta, eps: float, y32=None, lds: int | None = None):
+    """LayerNorm -> e4m3 codes [R, C] (uint8) + scales [C/128, lds] (elementwise.cuh layernorm_e4m3_kernel)."""
+    import torch
+    R, C = x.shape
+    y8 = torch.zeros(R, C, dtype=torch.uint8, device=x.device)
+    ys = torch.full((C // 128, lds or R), float("nan"), device=x.device)
+    call("probe_layernorm_e4m3", x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y8.data_ptr(), ys.data_ptr(),
+         ys.stride(0), ptr(y32), R, C, eps, stream())
+    return y8, ys
 
 
 # ------------------------------------------------------------------------------------------------ fp64 references

@@ -177,27 +177,3 @@ def test_block_scales_struct_and_config_sizes_match_c(tmp_path):
 def test_abi_version_counts_the_fp8_fields(built_lib):
     assert built_lib.thmr_abi_version() >= 6
 
-
-def test_fp8_probe_builds_and_exports_every_bound_wrapper(built_lib):
-    """The FP8 mode's test-only probe (tests/csrc/fp8_probe.cu) builds with the library, loads on a CPU-only host and
-    exports exactly the wrappers tests/fp8_probe.py binds, and nothing of the library's internals."""
-    import re
-    import shutil
-    import subprocess
-    import fp8_probe
-    from tokenhmr_b200 import _build
-    assert _build.FP8_PROBE_PATH == fp8_probe.PROBE_PATH and fp8_probe.PROBE_PATH.exists()
-    assert _build.FP8_PROBE_STAMP.read_text().strip() == _build.source_hash(probe=True)
-    src = (ROOT / "tests" / "csrc" / "fp8_probe.cu").read_text()
-    defined = set(re.findall(r"^FP8_PROBE_API\s+[\w\s\*]+?\b(fp8_probe_\w+)\s*\(", src, flags=re.M))
-    assert defined == set(fp8_probe.SIGNATURES), defined ^ set(fp8_probe.SIGNATURES)
-    L = fp8_probe.lib()
-    assert L.fp8_probe_gemm_desc_size() == ctypes.sizeof(fp8_probe.Fp8GemmDesc)
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("no nm")
-    out = subprocess.run([nm, "-D", "--defined-only", str(fp8_probe.PROBE_PATH)], check=True, capture_output=True,
-                         text=True).stdout
-    names = [ln.split()[-1] for ln in out.splitlines() if ln.strip()]
-    assert set(fp8_probe.SIGNATURES) <= set(names)
-    assert not [n for n in names if "thmr" in n]

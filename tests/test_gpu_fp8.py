@@ -3,7 +3,6 @@ and its e4m3 output epilogue), against the quantisation definition (exact) and f
 import pytest
 import torch
 
-import fp8_probe
 import probe
 from tokenhmr_b200 import fp8
 
@@ -21,7 +20,6 @@ C_BLK = 2.0 ** -10
 @pytest.fixture(autouse=True)
 def _flags(cuda_dev, built_lib):
     yield
-    assert fp8_probe.flags() == 0, "FP8 probe device flags set"
     assert probe.flags() == 0, "probe device flags set"
 
 
@@ -54,7 +52,7 @@ def test_layernorm_e4m3_matches_definition(cuda_dev):
     beta = 0.1 * torch.randn(C, device=cuda_dev, generator=g)
     beta[:128] = 0.0                             # row 7, group 0: amax = 0 -> scale 1, codes 0
     y32 = torch.full((R, C), float("nan"), device=cuda_dev)
-    y8, ys = fp8_probe.layernorm_e4m3(x, gamma, beta, 1e-6, y32=y32, lds=R + 24)
+    y8, ys = probe.layernorm_e4m3(x, gamma, beta, 1e-6, y32=y32, lds=R + 24)
     ref32 = torch.empty(R, C, device=cuda_dev)
     probe.call("probe_layernorm", x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), None, 0, ref32.data_ptr(), R, C,
                1e-6, 0, 0, probe.stream())
@@ -75,9 +73,9 @@ def _check_gemm(name, A, W, M, N, K, *, act="none", bias=None, resid=None, force
     if e4m3_out:
         out8 = torch.zeros(M, N, dtype=torch.uint8, device="cuda")
         out8_scale = torch.full((N // 128, M), float("nan"), device="cuda")
-    fp8_probe.gemm_fp8(qa, a_scale, qw, sw, M, N, K, bias=bias, resid=out32 if resid is not None else None,
-                   ldr=N if resid is not None else 0, act=act, out32=out32, ld32=N, out8=out8, out8_scale=out8_scale,
-                   force_bn=force_bn)
+    probe.gemm_fp8(qa, a_scale, qw, sw, M, N, K, bias=bias, resid=out32 if resid is not None else None,
+               ldr=N if resid is not None else 0, act=act, out32=out32, ld32=N, out8=out8, out8_scale=out8_scale,
+               force_bn=force_bn)
     torch.cuda.synchronize()
     Ad = fp8.dequantize_rows(qa, sa).double()
     Wd = fp8.dequantize_weight_blocks(qw, sw).double()
@@ -143,9 +141,9 @@ def test_gemm_fp8_chain_uses_epilogue_scales(cuda_dev):
     h8 = torch.zeros(M, F, dtype=torch.uint8, device=cuda_dev)
     hs = torch.ones(F // 128, (M + 127) // 128 * 128 + 128, device=cuda_dev)
     h32 = torch.empty(M, F, device=cuda_dev)
-    fp8_probe.gemm_fp8(qx, _pad_scales(sx, M), q1, s1, M, F, D, act="gelu", out32=h32, ld32=F, out8=h8, out8_scale=hs)
+    probe.gemm_fp8(qx, _pad_scales(sx, M), q1, s1, M, F, D, act="gelu", out32=h32, ld32=F, out8=h8, out8_scale=hs)
     y = torch.full((M, D), float("nan"), device=cuda_dev)
-    fp8_probe.gemm_fp8(h8, hs, q2, s2, M, D, F, out32=y, ld32=D)
+    probe.gemm_fp8(h8, hs, q2, s2, M, D, F, out32=y, ld32=D)
     torch.cuda.synchronize()
     hq, hsc = fp8.quantize_rows(h32)
     assert torch.equal(h8, hq.view(torch.uint8)) and torch.equal(hs[:, :M], hsc)

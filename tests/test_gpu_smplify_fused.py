@@ -31,6 +31,7 @@ import ctypes
 import pytest
 import torch
 
+import probe
 from oracle import smpl_oracle as S
 
 pytestmark = pytest.mark.gpu
@@ -49,48 +50,6 @@ def model(cuda_dev):
 def facade(model):
     from tokenhmr_b200.engine import _SmplFacade
     return _SmplFacade(model)
-
-
-class _SmplifyProbe:
-    """ctypes binding of tests/libthmr_smplify_probe.so (tests/csrc/smplify_probe.cu), built by _build.build()."""
-    SIGNATURES = {
-        "smplify_probe_last_error": (ctypes.c_char_p, []),
-        "probe_smplify_loss": (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 5),
-        "probe_smplify_adam": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_long, ctypes.c_int, ctypes.c_double,
-                                                                       ctypes.c_void_p]),
-    }
-
-    def __init__(self):
-        from pathlib import Path
-        import probe
-        path = Path(__file__).resolve().parent / "libthmr_smplify_probe.so"
-        if not path.exists():
-            raise RuntimeError(f"{path} not found: it is built by tokenhmr_b200._build.build()")
-        self.lib = ctypes.CDLL(str(path))
-        for name, (res, args) in self.SIGNATURES.items():
-            fn = getattr(self.lib, name)
-            fn.restype, fn.argtypes = res, args
-        self.assert_within = probe.assert_within
-
-    def call(self, name, *args):
-        status = getattr(self.lib, name)(*args)
-        if status != 0:
-            raise RuntimeError(f"{name} failed ({status}): "
-                               f"{self.lib.smplify_probe_last_error().decode(errors='replace')}")
-
-    @staticmethod
-    def stream():
-        return torch.cuda.current_stream().cuda_stream
-
-
-_PROBE = None
-
-
-def _probe():
-    global _PROBE
-    if _PROBE is None:
-        _PROBE = _SmplifyProbe()
-    return _PROBE
 
 
 def _fit_inputs(B, J, nb, seed):
@@ -115,7 +74,6 @@ def _fresh(t):
 @pytest.mark.parametrize("B", [1, 17, 64, 257])
 def test_loss_kernel_vs_fp64_autograd(cuda_dev, B):
     from tokenhmr_b200.fitting import camera_fitting_loss
-    P = _probe()
     J = 44
     g = torch.Generator(device="cuda").manual_seed(100 + B)
     joints = 0.4 * torch.randn(B, J, 3, device="cuda", generator=g)
@@ -131,12 +89,12 @@ def test_loss_kernel_vs_fp64_autograd(cuda_dev, B):
     gj = torch.empty(B, J, 3, device="cuda")
     gcam = torch.empty(B, 3, device="cuda")
     part = torch.empty(2, B, device="cuda")
-    P.call("probe_smplify_loss", joints.data_ptr(), cam.data_ptr(), focal.data_ptr(), kp2.data_ptr(), kp3.data_ptr(),
-           J, B, gj.data_ptr(), gcam.data_ptr(), part.data_ptr(), None, P.stream())
+    probe.call("probe_smplify_loss", joints.data_ptr(), cam.data_ptr(), focal.data_ptr(), kp2.data_ptr(),
+               kp3.data_ptr(), J, B, gj.data_ptr(), gcam.data_ptr(), part.data_ptr(), None, probe.stream())
     pj2d = torch.empty(B, J, 2, device="cuda")
     part_f = torch.empty(2, B, device="cuda")
-    P.call("probe_smplify_loss", joints.data_ptr(), cam.data_ptr(), focal.data_ptr(), kp2.data_ptr(), kp3.data_ptr(),
-           J, B, None, None, part_f.data_ptr(), pj2d.data_ptr(), P.stream())
+    probe.call("probe_smplify_loss", joints.data_ptr(), cam.data_ptr(), focal.data_ptr(), kp2.data_ptr(),
+               kp3.data_ptr(), J, B, None, None, part_f.data_ptr(), pj2d.data_ptr(), probe.stream())
     torch.cuda.synchronize()
     assert torch.equal(pj2d, u32), "projection differs from the same fp32 operations in torch"
     assert torch.equal(part_f, part)
@@ -170,12 +128,12 @@ def test_loss_kernel_vs_fp64_autograd(cuda_dev, B):
     keep = ~near_zero
     keep_s = keep.all(1)
     rep = {}
-    P.assert_within(f"grad_joints B={B}", gj[keep], want_j[keep], bound_j[keep], rep)
+    probe.assert_within(f"grad_joints B={B}", gj[keep], want_j[keep], bound_j[keep], rep)
     if bool(keep_s.any()):
-        P.assert_within(f"grad_cam B={B}", gcam[keep_s], want_c[keep_s], bound_c[keep_s], rep)
-    P.assert_within(f"fit2D_b B={B}", part[0], fit_b.detach(), 16 * U * (mag + r2).sum(1) + J * U * r2.sum(1), rep)
-    P.assert_within(f"push3D_b B={B}", part[1], push_b.detach(),
-                    16 * U * (j64.detach().abs().sum(-1) + k3.abs().sum(-1) + r3).sum(1) + J * U * r3.sum(1), rep)
+        probe.assert_within(f"grad_cam B={B}", gcam[keep_s], want_c[keep_s], bound_c[keep_s], rep)
+    probe.assert_within(f"fit2D_b B={B}", part[0], fit_b.detach(), 16 * U * (mag + r2).sum(1) + J * U * r2.sum(1), rep)
+    probe.assert_within(f"push3D_b B={B}", part[1], push_b.detach(),
+                        16 * U * (j64.detach().abs().sum(-1) + k3.abs().sum(-1) + r3).sum(1) + J * U * r3.sum(1), rep)
     print(f"[smplify loss] B={B}: {n_excl} joints with a 2D residual within rounding of zero excluded "
           f"({int((~keep_s).sum())} samples' pred_cam_t cotangent); worst err/bound "
           + ", ".join(f"{k} {v:.3g}" for k, v in rep.items()))
@@ -186,7 +144,6 @@ def test_loss_kernel_vs_fp64_autograd(cuda_dev, B):
 def test_adam_kernel_equals_torch_adam_bitwise(cuda_dev, lr):
     """20 steps of identical random gradients (magnitudes 1e-6 .. 1e3, some exact zeros) on the three parameter sets:
     every parameter, after every step, bit for bit equal to torch.optim.Adam's default (foreach) CUDA step."""
-    P = _probe()
     B = 64
     g = torch.Generator(device="cuda").manual_seed(7)
     go = torch.randn(B, 1, 3, 3, device="cuda", generator=g)
@@ -205,8 +162,8 @@ def test_adam_kernel_equals_torch_adam_bitwise(cuda_dev, lr):
             t.grad = gr.clone()
         opt.step()
         gflat = torch.cat([grads[1].flatten(), grads[0].flatten(), grads[2].flatten()])
-        P.call("probe_smplify_adam", flat.data_ptr(), m.data_ptr(), v.data_ptr(), gflat.data_ptr(), flat.numel(), step,
-               lr, P.stream())
+        probe.call("probe_smplify_adam", flat.data_ptr(), m.data_ptr(), v.data_ptr(), gflat.data_ptr(), flat.numel(),
+                   step, lr, probe.stream())
         torch.cuda.synchronize()
         for name, got, want in (("global_orient", flat[:n1], params[1]), ("body_pose", flat[n1:n2], params[0]),
                                 ("pred_cam_t", flat[n2:], params[2])):

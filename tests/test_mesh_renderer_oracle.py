@@ -1,12 +1,12 @@
 """The prediction grid's oracle (oracle/openpose_oracle.py) and the overlay's span generator (csrc/keypoints.cuh, run on
-the host through tests/libthmr_pose_probe.so) against live OpenCV, and the grid golden (written from the live
+the host through tests/libthmr_probe.so) against live OpenCV, and the grid golden (written from the live
 mesh_renderer.py, render_openpose.py, cv2 and make_grid) against the oracle.  No GPU."""
-import ctypes
 import hashlib
 
 import numpy as np
 import pytest
 
+import probe
 from oracle import openpose_oracle as O
 
 GOLD = "mesh_renderer_reference.npz"
@@ -46,17 +46,7 @@ def test_primitive_restatement_matches_live_cv2():
     assert not bad, f"{len(bad)} of 10000 primitives differ from cv2, first {bad[:3]}"
 
 
-@pytest.fixture(scope="module")
-def pose_probe(built_lib):
-    from tokenhmr_b200 import _build
-    L = ctypes.CDLL(str(_build.POSE_PROBE_PATH))
-    L.probe_pose_draw.restype = ctypes.c_int
-    L.probe_pose_draw.argtypes = [ctypes.c_int] + [ctypes.c_longlong] * 4 + [ctypes.c_int, ctypes.c_int,
-                                                                             ctypes.c_void_p]
-    return L
-
-
-def test_span_generator_matches_live_cv2(pose_probe):
+def test_span_generator_matches_live_cv2(built_lib):
     """The __host__ __device__ span generator the raster kernel runs, on the host."""
     cv2 = pytest.importorskip("cv2")
     bad = []
@@ -67,7 +57,7 @@ def test_span_generator_matches_live_cv2(pose_probe):
               (0, (0, 0), (0, 0), 1, 1), (0, (-2, 3), (-2, 300), 4, 9), (0, (3, 3), (4, 3), 8, 8)]
     for kind, p0, p1, W, H in cases:
         m = np.zeros((H, W), np.uint8)
-        assert pose_probe.probe_pose_draw(kind, p0[0], p0[1], p1[0], p1[1], W, H, m.ctypes.data) == 0
+        assert probe.lib().probe_pose_draw(kind, p0[0], p0[1], p1[0], p1[1], W, H, m.ctypes.data) == 0
         if not np.array_equal(m, _cv2_mask(cv2, kind, p0, p1, W, H)):
             bad.append((kind, p0, p1, W, H))
     assert not bad, f"{len(bad)} of {len(cases)} primitives differ from cv2, first {bad[:3]}"

@@ -1,5 +1,5 @@
-"""The test-only kernel probe (tests/csrc/kernel_probe.cu) builds with the library, loads on a CPU-only host and exports
-exactly the wrappers tests/probe.py binds (no compute calls here)."""
+"""The test-only probe library (tests/csrc/kernel_probe.cu) builds with the library, loads on a CPU-only host and
+exports exactly the wrappers tests/probe.py binds (no compute calls here)."""
 import ctypes
 import re
 from pathlib import Path
@@ -22,9 +22,9 @@ def test_probe_builds_and_exports_every_bound_wrapper(built_lib):
 
 
 def test_probe_keeps_the_library_internals_private(built_lib):
-    """Only the probe_* wrappers are exported: the probe compiles the same inline launchers as the library, and a shared
-    symbol would let one library's static state (e.g. a launcher's 'kernel attributes configured' flag) stand in for
-    the other's."""
+    """Every bound wrapper and none of the library's internals are exported: the probe compiles the same inline
+    launchers as the library, and a shared symbol would let one library's static state (e.g. a launcher's 'kernel
+    attributes configured' flag) stand in for the other's."""
     import shutil
     import subprocess
     nm = shutil.which("nm")
@@ -34,5 +34,6 @@ def test_probe_keeps_the_library_internals_private(built_lib):
     out = subprocess.run([nm, "-D", "--defined-only", str(probe.PROBE_PATH)], check=True, capture_output=True,
                          text=True).stdout
     names = [ln.split()[-1] for ln in out.splitlines() if ln.strip()]
+    assert set(probe.SIGNATURES) <= set(names), set(probe.SIGNATURES) - set(names)
     leaked = [n for n in names if "thmr" in n]
     assert not leaked, leaked[:10]

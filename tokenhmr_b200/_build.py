@@ -1,8 +1,7 @@
 """Builds libtokenhmr_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU), and next to the test suite
-the kernel probes tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers),
-tests/libthmr_fp8_probe.so (tests/csrc/fp8_probe.cu: the same for the FP8 mode's kernels),
-tests/libthmr_pose_probe.so (tests/csrc/pose_probe.cu: the skeleton overlay's span generator, run on the host) and
-tests/libthmr_smplify_probe.so (tests/csrc/smplify_probe.cu: the fused SMPLify-inverse's loss and Adam kernels)."""
+the probe library tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers
+of every mode, the fused SMPLify-inverse's loss and Adam kernels, and the skeleton overlay's span generator run on the
+host)."""
 from __future__ import annotations
 
 import hashlib
@@ -18,15 +17,6 @@ STAMP = PKG_DIR / ".libtokenhmr_b200.stamp"
 PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "kernel_probe.cu"
 PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_probe.so"
 PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_probe.stamp"
-FP8_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "fp8_probe.cu"
-FP8_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_fp8_probe.so"
-FP8_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_fp8_probe.stamp"
-POSE_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "pose_probe.cu"
-POSE_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_pose_probe.so"
-POSE_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_pose_probe.stamp"
-SMPLIFY_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "smplify_probe.cu"
-SMPLIFY_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_smplify_probe.so"
-SMPLIFY_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_smplify_probe.stamp"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -76,22 +66,13 @@ def _compile(src: Path, out: Path, stamp: Path, flags: list, want: str, force: b
 
 
 def build_probe(force: bool = False, verbose: bool = False) -> Path:
-    """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so, tests/csrc/fp8_probe.cu ->
-    tests/libthmr_fp8_probe.so, tests/csrc/pose_probe.cu -> tests/libthmr_pose_probe.so and tests/csrc/smplify_probe.cu
-    -> tests/libthmr_smplify_probe.so (no-op when sources are unchanged)."""
-    want = source_hash(probe=True)
-    if FP8_PROBE_SRC.exists():
-        _compile(FP8_PROBE_SRC, FP8_PROBE_PATH, FP8_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
-    if POSE_PROBE_SRC.exists():
-        _compile(POSE_PROBE_SRC, POSE_PROBE_PATH, POSE_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
-    if SMPLIFY_PROBE_SRC.exists():
-        _compile(SMPLIFY_PROBE_SRC, SMPLIFY_PROBE_PATH, SMPLIFY_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force,
-                 verbose)
-    return _compile(PROBE_SRC, PROBE_PATH, PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, want, force, verbose)
+    """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so (no-op when sources are unchanged)."""
+    return _compile(PROBE_SRC, PROBE_PATH, PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, source_hash(probe=True), force,
+                    verbose)
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile csrc/tokenhmr_b200.cu -> libtokenhmr_b200.so, and the kernel probe when the test sources are present
+    """Compile csrc/tokenhmr_b200.cu -> libtokenhmr_b200.so, and the probe library when the test sources are present
     (no-op when sources are unchanged)."""
     path = _compile(CSRC / "tokenhmr_b200.cu", LIB_PATH, STAMP, NVCC_FLAGS, source_hash(), force, verbose)
     if PROBE_SRC.exists():
