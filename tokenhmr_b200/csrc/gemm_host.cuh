@@ -13,6 +13,7 @@ struct GemmPlan {
   int grid;
   int cluster;   // 2: CTA pairs sharing the B tile (gemm_wgmma.cuh)
   int fp8;       // e4m3 operands (gemm_make_plan_fp8)
+  int epi;       // epilogue kind (kEpi*, gemm_wgmma.cuh)
 };
 
 struct GemmDesc {
@@ -34,6 +35,7 @@ struct GemmDesc {
   float screen_rel = 0.f, screen_abs = 0.f; int screen_row0 = 0;
   const int* row_map = nullptr; const int* m_dev = nullptr; int m_dev_off = 0;
   int force_bn = 0;   // 32 / 64 / 128 / 256, or 512 = a CTA pair (2-CTA cluster) on a 256 x 256 tile
+  int force_epi = 0;  // 0: the plan picks the epilogue kind; 1 + kEpi*: that kind (a specialised one only where it fits)
   unsigned long long* stamp = nullptr;   // in-graph start stamp slot (nullable)
   // FP8 (GemmParams): A and B point to e4m3 bytes (lda / ldb in elements = bytes), K a multiple of 128; block_n 64 or
   // 128, 128 with out8.  a_scale [K / 128][ld_as] must hold the tile-padded rows (ld_as >= M rounded up to 128).
@@ -46,12 +48,14 @@ struct GemmDesc {
 // Tile width: wide tiles move fewer operand bytes per MAC (every k-block moves (128 + BN) * 128 bytes for
 // 128 * BN * 64 MACs), so they win unless they leave SMs idle or their epilogue dominates.  Cost model per tile in
 // cycles on an H100 SM: per k-block max(MMA at 2048 fp16 MAC/clk, operand feed at ~32 B/clk from L2) plus a fixed
-// overhead, plus the epilogue.  The epilogue terms are fitted to the ViT GEMMs (M = 12288) on an H100 80GB HBM3 at a
-// 400 W power limit, so that the model picks the measured-faster width at all five of them: ~28 us per 128 x 256
-// tile (eight 32-column staging chunks) against ~3.5 us per 128 x 128 tile (two 64-column chunks), so 256 wins only
-// at long K (fc2, K = 5120); the narrower tiles are scaled from 128.  The row arg-min epilogue (VQ) is not staged and
-// is not charged.
-inline int pick_bn(int M, int N, int K, bool staged_epilogue, int force) {
+// overhead, plus the epilogue.  The epilogue terms are fitted to the ViT GEMMs (M = 12288) on an H100 80GB HBM3 (700 W
+// power limit; scripts/gemm_anatomy.py, per-tile timeline at K = 64), so that the model picks the measured-faster width
+// at all five of them.  The specialised epilogue kinds (fast_epilogue, block_n 128 / 256 only) cost 2.3-3.6 us per
+// 128 x 128 tile and 4-8 us per 128 x 256 tile (fp16 outputs; the fp32 residual ones move twice the bytes), ~5000
+// cycles per 128 columns, so 256 wins at all five.  The general epilogue costs ~30 us per 128 x 256 tile (eight
+// 32-column chunks) against ~7 us per 128 x 128 tile; the narrower tiles are scaled from 128.  The row arg-min
+// epilogue (VQ) is not staged and is not charged.
+inline int pick_bn(int M, int N, int K, bool staged_epilogue, bool fast_epilogue, int force) {
   if (force) return force;
   const int sms = num_sms();
   const int tm = (M + kGemmBM - 1) / kGemmBM;
@@ -65,7 +69,10 @@ inline int pick_bn(int M, int N, int K, bool staged_epilogue, int force) {
     const long waves = (tiles + sms - 1) / sms;
     const double mma = 4.0 * bn;
     const double feed = (128.0 + bn) * 128.0 / 32.0;
-    const double epilogue = !staged_epilogue ? 0.0 : bn == 256 ? 55000.0 : 7000.0 * bn / 128;
+    const double epilogue = !staged_epilogue                 ? 0.0
+                            : fast_epilogue && bn >= 128      ? 5000.0 * bn / 128
+                            : bn == 256                       ? 55000.0
+                                                              : 7000.0 * bn / 128;
     const double cost = waves * (num_kb * ((mma > feed ? mma : feed) + 40.0) + epilogue);
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = bn; }
   }
@@ -92,6 +99,23 @@ inline int pick_bn_fp8(int M, int N, int K) {
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = bn; }
   }
   return best;
+}
+
+// Epilogue kind of a plain fp16 GEMM: a specialised kind (gemm_epilogue_kind) where the descriptor asks for exactly its
+// operations and every base and pitch it touches allows 16-byte row vectors, else kEpiGeneral.  Only the 128- and
+// 256-wide tiles, where the ViT's GEMMs run, have the specialised kernels.
+inline int gemm_pick_epi(const GemmDesc& d, int bn, int cluster) {
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if ((bn != 128 && bn != 256) || cluster != 1 || d.argmin_out || d.resid_mod || d.seq_pitch || d.act32 || !al16(d.bias))
+    return kEpiGeneral;
+  if (d.out16 && !d.out32 && !d.resid && d.ld16 % 8 == 0 && al16(d.out16)) {
+    if (d.act == kActNone) return d.bias ? kEpiBiasF16 : kEpiF16;
+    if (d.act == kActGelu && d.bias) return kEpiBiasGeluF16;
+  }
+  if (d.out32 && !d.out16 && d.resid && d.bias && d.act == kActNone && d.ld32 % 4 == 0 && al16(d.out32) &&
+      d.ldr % 4 == 0 && al16(d.resid))
+    return kEpiBiasResidF32;
+  return kEpiGeneral;
 }
 
 inline int make_tmap_2d_e4m3(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
@@ -126,9 +150,11 @@ inline int gemm_make_plan_fp8(const GemmDesc& d, GemmPlan* plan) {
   p.out8 = d.out8; p.ld8 = d.ld8; p.out8_scale = d.out8_scale; p.ld8s = d.ld8s;
   THMR_TRY(make_tmap_2d_e4m3(&plan->tmA, d.A, d.a_rows, d.K, d.lda, kGemmBM, 128));
   THMR_TRY(make_tmap_2d_e4m3(&plan->tmB, d.B, d.N, d.K, d.ldb, bn, 128));
+  THMR_CHECK(d.force_epi == 0 || d.force_epi == 1 + kEpiGeneral, "gemm fp8: general epilogue only");
   plan->bn = bn;
   plan->cluster = 1;
   plan->fp8 = 1;
+  plan->epi = kEpiGeneral;
   const long tiles_m = (d.M + kGemmBM - 1) / kGemmBM;
   const long tiles = tiles_m * ((d.N + bn - 1) / bn);
   p.m_fast = (tiles_m > 1 && d.M < d.N) ? 1 : 0;
@@ -143,7 +169,8 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   THMR_CHECK(d.out32 || d.out16 || d.argmin_out, "gemm: no output");
   const int cluster = d.force_bn == 512 ? 2 : 1;
   THMR_CHECK(cluster == 1 || !d.argmin_out, "gemm: block_n 512 (CTA pair) does not support the arg-min modes");
-  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.K, d.argmin_out == nullptr, d.force_bn);
+  const bool fast_epi = gemm_pick_epi(d, 256, cluster) != kEpiGeneral;   // the kind does not depend on the width
+  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.K, d.argmin_out == nullptr, fast_epi, d.force_bn);
   THMR_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: bad block_n %d", bn);
   GemmParams& p = plan->p;
   memset(&p, 0, sizeof(p));
@@ -174,6 +201,10 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   plan->bn = bn;
   plan->cluster = cluster;
   plan->fp8 = 0;
+  plan->epi = gemm_pick_epi(d, bn, cluster);
+  THMR_CHECK(d.force_epi == 0 || d.force_epi - 1 == kEpiGeneral || d.force_epi - 1 == plan->epi,
+             "gemm: epilogue kind %d does not fit this GEMM (its kind is %d)", d.force_epi - 1, plan->epi);
+  if (d.force_epi) plan->epi = d.force_epi - 1;
   const long tiles_m = (d.M + kGemmBM * cluster - 1) / (kGemmBM * cluster);
   const long tiles = d.argmin_out ? tiles_m : tiles_m * ((d.N + bn - 1) / bn);
   // the CTAs of a wave should share tiles of the larger operand (TileIter)
@@ -183,13 +214,13 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   return THMR_OK;
 }
 
-template <int BN, int STAGES, int CLUSTER = 1, bool FP8 = false>
+template <int BN, int STAGES, int CLUSTER = 1, bool FP8 = false, int EPI = kEpiGeneral, bool TIMELINE = false>
 inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
   using S = GemmSmem<BN, STAGES, FP8>;
   static_assert(S::kTotal <= 232448, "GEMM shared memory exceeds 227 KB");
   static bool configured = false;
   if (!configured) {
-    THMR_CUDA(cudaFuncSetAttribute(gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    THMR_CUDA(cudaFuncSetAttribute(gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8, EPI, TIMELINE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    S::kTotal));
     configured = true;
   }
@@ -205,11 +236,24 @@ inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8>, plan.tmA, plan.tmB, plan.p));
+  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8, EPI, TIMELINE>, plan.tmA, plan.tmB, plan.p));
   return THMR_OK;
 }
 
-inline int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+template <int BN, int STAGES, bool TIMELINE>
+inline int gemm_launch_epi(const GemmPlan& plan, cudaStream_t stream) {
+  switch (plan.epi) {
+    case kEpiGeneral: return gemm_launch_t<BN, STAGES, 1, false, kEpiGeneral, TIMELINE>(plan, stream);
+    case kEpiF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiF16, TIMELINE>(plan, stream);
+    case kEpiBiasF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasF16, TIMELINE>(plan, stream);
+    case kEpiBiasGeluF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasGeluF16, TIMELINE>(plan, stream);
+    case kEpiBiasResidF32: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasResidF32, TIMELINE>(plan, stream);
+  }
+  return fail(THMR_ERR_INVALID, "gemm: unsupported epilogue kind %d", plan.epi);
+}
+
+// Launches a plan made by gemm_make_plan / gemm_make_plan_fp8.
+inline int gemm_launch_plain(const GemmPlan& plan, cudaStream_t stream) {
   if (plan.fp8) {
     // the stage ring also carries 512 bytes of activation scales per stage, and the epilogue the row scales
     if (plan.bn == 128) return gemm_launch_t<128, 5, 1, true>(plan, stream);
@@ -218,12 +262,27 @@ inline int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
   }
   if (plan.cluster == 2) return gemm_launch_t<256, 4, 2>(plan, stream);
   switch (plan.bn) {
-    case 256: return gemm_launch_t<256, 4>(plan, stream);
-    case 128: return gemm_launch_t<128, 6>(plan, stream);
+    case 256: return gemm_launch_epi<256, 4, false>(plan, stream);
+    case 128: return gemm_launch_epi<128, 6, false>(plan, stream);
     case 64: return gemm_launch_t<64, 8>(plan, stream);
     case 32: return gemm_launch_t<32, 8>(plan, stream);
   }
   return fail(THMR_ERR_INVALID, "gemm: unsupported block_n %d", plan.bn);
+}
+
+// gemm_launch<true>: the per-tile timeline kernels (GemmParams::timeline, test probe only), fp16 single-CTA plans at
+// block_n 128 / 256
+template <bool TIMELINE = false>
+inline int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+  if constexpr (TIMELINE) {
+    THMR_CHECK(!plan.fp8 && plan.cluster == 1 && (plan.bn == 128 || plan.bn == 256),
+               "gemm timeline: fp16 block_n 128 / 256 only (block_n %d)", plan.bn);
+    return plan.bn == 256 ? gemm_launch_epi<256, 4, true>(plan, stream) : gemm_launch_epi<128, 6, true>(plan, stream);
+  } else {
+    THMR_CHECK(plan.epi == kEpiGeneral || (plan.bn >= 128 && plan.cluster == 1 && !plan.fp8),
+               "gemm: epilogue kind %d at block_n %d", plan.epi, plan.bn);
+    return gemm_launch_plain(plan, stream);
+  }
 }
 
 }  // namespace thmr

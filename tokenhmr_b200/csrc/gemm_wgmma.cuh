@@ -30,6 +30,14 @@ namespace thmr {
 
 enum : int { kActNone = 0, kActGelu = 1, kActRelu = 2 };
 
+// Epilogue kinds (GemmPlan::epi, a template parameter of the kernel).  kEpiGeneral (gemm_epilogue_rows) compiles every
+// option of GemmParams in; the others compile only what the ViT's call sites use (gemm_epilogue_kind):
+//   kEpiF16           alpha * acc -> fp16                          decoder to_kv
+//   kEpiBiasF16       alpha * acc + bias -> fp16                   QKV
+//   kEpiBiasGeluF16   GELU(alpha * acc + bias) -> fp16             fc1
+//   kEpiBiasResidF32  alpha * acc + bias + resid -> fp32           proj, fc2 (resid aliases out32)
+enum : int { kEpiGeneral = 0, kEpiF16 = 1, kEpiBiasF16 = 2, kEpiBiasGeluF16 = 3, kEpiBiasResidF32 = 4 };
+
 struct GemmParams {
   int M, N, K;
   float* out32;   // acc + bias + resid, fp32 (nullable)
@@ -81,6 +89,12 @@ struct GemmParams {
   int ld8;
   float* out8_scale;
   int ld8s;
+  // per-tile phase timeline (gemm_f16_tn_kernel<..., TIMELINE = true>, test probe only): lane 0 of each consumer
+  // warpgroup writes four %globaltimer stamps per tile into timeline[cta][slot][wg][4] (tile start, first full barrier
+  // passed, last wgmma retired, epilogue done) for the CTA's first timeline_slots tiles, and %smid into timeline_sm[cta]
+  unsigned long long* timeline;
+  int timeline_slots;
+  int* timeline_sm;
 };
 
 // Tile order shared by the producer and the consumers.  Normal mode: tiles round-robin over CTAs, column tile
@@ -158,7 +172,8 @@ __device__ __forceinline__ float gelu_erf(float x) {
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(p));   // 1 ulp-class MUFU reciprocal (p >= 1; p = inf -> 0)
   const float e = 1.0f - r;                       // erf(|x| / sqrt(2))
-  return 0.5f * x + 0.5f * fabsf(x) * e;          // 0.5 x (1 + sign(x) e)
+  // 0.5 x (1 + sign(x) e) as fma(x, 0.5, (0.5 |x|) e), spelled out so that every epilogue kind rounds it alike
+  return fmaf(x, 0.5f, __fmul_rn(__fmul_rn(fabsf(x), 0.5f), e));
 }
 
 template <int BN>
@@ -180,6 +195,26 @@ __device__ __forceinline__ float gemm_act(int act, float v) {
 }
 
 __device__ __forceinline__ bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+// Fragment -> staging block: the accumulators of chunk c (columns c * CH ..) of the thread's rows fr, fr + 8 of the
+// warpgroup's 64, in the swizzled staging layout of gemm_epilogue_rows.  c must be a compile-time constant after
+// unrolling, so that acc is indexed by constants and stays in registers.
+template <int BN>
+__device__ __forceinline__ void gemm_stage_chunk(const float (&acc)[BN / 2], int c, uint32_t stage, int fr, int fswz,
+                                                 int lane) {
+  constexpr int CH = gemm_chunk<BN>();
+  constexpr int OCT = CH / 8;
+#pragma unroll
+  for (int j = 0; j < OCT; ++j) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int u = 2 * j + ((lane & 3) >> 1);
+      const int a = 4 * (c * OCT + j) + 2 * i;
+      sts_f32x2(stage + 4 * ((fr + 8 * i) * CH + (((u & ~7) | ((u ^ fswz) & 7)) << 2) + 2 * (lane & 1)), acc[a],
+                acc[a + 1]);
+    }
+  }
+}
 
 // Element-wise epilogue of one consumer warpgroup: its 64 rows x BN columns of accumulators, rows m0w.. of the output.
 // The accumulator fragment (two rows x two columns per 8-column group and thread) goes to a shared-memory chunk of
@@ -229,16 +264,7 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
 
 #pragma unroll
   for (int c = 0; c < BN / CH; ++c) {
-#pragma unroll
-    for (int j = 0; j < OCT; ++j) {
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int u = 2 * j + ((lane & 3) >> 1);
-        const int a = 4 * (c * OCT + j) + 2 * i;
-        sts_f32x2(stage + 4 * ((fr + 8 * i) * CH + (((u & ~7) | ((u ^ fswz) & 7)) << 2) + 2 * (lane & 1)), acc[a],
-                  acc[a + 1]);
-      }
-    }
+    gemm_stage_chunk<BN>(acc, c, stage, fr, fswz, lane);
     named_barrier_sync(bar_id, 128);
 
     const int ccol = n0 + c * CH + 8 * (lane >> 3);   // first column of octet 0 of this thread in the chunk
@@ -286,12 +312,13 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
         v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
       }
       // alpha * acc + bias + resid, mask, activation: the operation order of the reference epilogue, element for element
+      // (rounded step by step, never contracted: gemm_epilogue_kind computes the same values)
       if (!final_vals) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          v[e] *= p.alpha;
-          if (p.bias) v[e] += bias[k >> 1][e];
-          if (p.resid) v[e] += res[k][e];
+          v[e] = __fmul_rn(v[e], p.alpha);
+          if (p.bias) v[e] = __fadd_rn(v[e], bias[k >> 1][e]);
+          if (p.resid) v[e] = __fadd_rn(v[e], res[k][e]);
           if (!keep[ri]) v[e] = 0.f;
           if (p.act32) v[e] = gemm_act(p.act, v[e]);
         }
@@ -349,6 +376,130 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
   }
 }
 
+// The octet of a partial column tile (col < N < col + 8) of gemm_epilogue_kind, element by element.
+template <int EPI>
+__device__ __forceinline__ void gemm_epilogue_kind_tail(const GemmParams& p, const float (&v)[8], int row, int col) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    if (col + e >= p.N) break;
+    float x = __fmul_rn(v[e], p.alpha);
+    if constexpr (EPI != kEpiF16) x = __fadd_rn(x, __ldg(p.bias + col + e));
+    if constexpr (EPI == kEpiBiasResidF32) {
+      const size_t i = static_cast<size_t>(row) * p.ld32 + col + e;
+      p.out32[i] = __fadd_rn(x, p.resid[static_cast<size_t>(row) * p.ldr + col + e]);
+    } else {
+      if constexpr (EPI == kEpiBiasGeluF16) x = gelu_erf(x);
+      p.out16[static_cast<size_t>(row) * p.ld16 + col + e] = __float2half_rn(x);
+    }
+  }
+}
+
+// Element-wise epilogue of one consumer warpgroup for a specialised kind (kEpiF16 .. kEpiBiasResidF32): the staging
+// and the row walk of gemm_epilogue_rows and the same values element for element, but only the kind's operations are
+// compiled, and the chunks go through one rolled loop, so that the walk is emitted once instead of once per chunk.
+// Only the fragment staging is unrolled per chunk (a uniform branch picks it), since it indexes registers.  The plan
+// (gemm_make_plan) guarantees 16-byte aligned bases and pitches for every operand the kind touches.
+template <int BN, int EPI>
+__device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
+                                                   int m0w, int n0, int M_eff, uint32_t bar_id) {
+  constexpr bool kBias = EPI != kEpiF16;
+  constexpr bool kResid = EPI == kEpiBiasResidF32;
+  constexpr int CH = gemm_chunk<BN>();
+  constexpr int OCT = CH / 8;
+  constexpr int ITEMS = OCT / 2;
+  const int lane = threadIdx.x & 31;
+  const int w4 = (threadIdx.x >> 5) & 3;
+  const int fr = w4 * 16 + (lane >> 2);
+  const int fswz = (((lane >> 2) & 3) << 1) | ((lane >> 4) & 1);
+  const int rswz = ((lane & 3) << 1) | ((lane >> 2) & 1);
+#pragma unroll 1
+  for (int c = 0; c < BN / CH; ++c) {
+#pragma unroll
+    for (int cc = 0; cc < BN / CH; ++cc)
+      if (cc == c) gemm_stage_chunk<BN>(acc, cc, stage, fr, fswz, lane);
+    named_barrier_sync(bar_id, 128);
+
+    // item k: row 8 (w4 + 4 (k % 2)) + lane % 8 of the warpgroup, octet 4 (k / 2) + lane / 8 of the chunk
+    const int ccol = n0 + c * CH + 8 * (lane >> 3);
+    float bias[ITEMS / 2][8];
+    float res[ITEMS][8];
+    if constexpr (kBias && !(kResid && ITEMS == 2)) {
+#pragma unroll
+      for (int ob = 0; ob < ITEMS / 2; ++ob) {
+        const int col = ccol + 32 * ob;
+        if (col + 8 <= p.N) {
+          const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+          const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
+          bias[ob][0] = b0.x; bias[ob][1] = b0.y; bias[ob][2] = b0.z; bias[ob][3] = b0.w;
+          bias[ob][4] = b1.x; bias[ob][5] = b1.y; bias[ob][6] = b1.z; bias[ob][7] = b1.w;
+        }
+      }
+    }
+    if constexpr (kResid) {
+      // all residual loads of the chunk before any of its stores
+#pragma unroll
+      for (int k = 0; k < ITEMS; ++k) {
+        const int row = m0w + 8 * (w4 + 4 * (k & 1)) + (lane & 7);
+        const int col = ccol + 32 * (k >> 1);
+        if (row < M_eff && col + 8 <= p.N) {
+          const float* r = p.resid + static_cast<size_t>(row) * p.ldr + col;
+          const float4 x0 = *reinterpret_cast<const float4*>(r);
+          const float4 x1 = *reinterpret_cast<const float4*>(r + 4);
+          res[k][0] = x0.x; res[k][1] = x0.y; res[k][2] = x0.z; res[k][3] = x0.w;
+          res[k][4] = x1.x; res[k][5] = x1.y; res[k][6] = x1.z; res[k][7] = x1.w;
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const int lr = 8 * (w4 + 4 * (k & 1)) + (lane & 7);
+      const int oct = 4 * (k >> 1) + (lane >> 3);
+      const int row = m0w + lr;
+      const int col = ccol + 32 * (k >> 1);
+      if (row >= M_eff || col >= p.N) continue;
+      float v[8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int u = 2 * oct + h;
+        const float4 s = lds_f32x4(stage + 4 * (lr * CH + (((u & ~7) | ((u ^ rswz) & 7)) << 2)));
+        v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
+      }
+      if (col + 8 > p.N) {
+        gemm_epilogue_kind_tail<EPI>(p, v, row, col);
+        continue;
+      }
+      if constexpr (kResid && ITEMS == 2) {
+        // 128 accumulators stay live across the rolled chunk loop: the 32-column chunks of BN = 256 have no registers
+        // left to hold the bias from before the residual loads, so it is read here
+        const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+        const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
+        bias[0][0] = b0.x; bias[0][1] = b0.y; bias[0][2] = b0.z; bias[0][3] = b0.w;
+        bias[0][4] = b1.x; bias[0][5] = b1.y; bias[0][6] = b1.z; bias[0][7] = b1.w;
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[e] = __fmul_rn(v[e], p.alpha);
+        if constexpr (kBias) v[e] = __fadd_rn(v[e], bias[k >> 1][e]);
+        if constexpr (kResid) v[e] = __fadd_rn(v[e], res[k][e]);
+        if constexpr (EPI == kEpiBiasGeluF16) v[e] = gelu_erf(v[e]);
+      }
+      if constexpr (kResid) {
+        float4* o = reinterpret_cast<float4*>(p.out32 + static_cast<size_t>(row) * p.ld32 + col);
+        o[0] = make_float4(v[0], v[1], v[2], v[3]);
+        o[1] = make_float4(v[4], v[5], v[6], v[7]);
+      } else {
+        uint4 q;
+        __half2* h2 = reinterpret_cast<__half2*>(&q);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) h2[e] = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
+        *reinterpret_cast<uint4*>(p.out16 + static_cast<size_t>(row) * p.ld16 + col) = q;
+      }
+    }
+    // the next chunk (or tile) overwrites the staging block
+    named_barrier_sync(bar_id, 128);
+  }
+}
+
 // e4m3 output, before the element-wise epilogue: replaces the thread's accumulators by v = act(alpha * acc + bias) and
 // derives each tile row's scale from the amax of all its BN = 128 columns (the four lanes of a quad hold one row), so
 // that no code of a row is written before its whole 128-column group has been seen.  The scale goes to out8_scale,
@@ -382,7 +533,7 @@ __device__ __forceinline__ void gemm_row_scales_e4m3(const GemmParams& p, float 
   }
 }
 
-template <int BN, int STAGES, int CLUSTER, bool FP8 = false>
+template <int BN, int STAGES, int CLUSTER, bool FP8 = false, int EPI = kEpiGeneral, bool TIMELINE = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using S = GemmSmem<BN, STAGES, FP8>;
@@ -390,6 +541,8 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
   static_assert(CLUSTER == 1 || (CLUSTER == 2 && BN >= 128), "cluster pairs split B in two halves of >= 64 rows");
   static_assert(!FP8 || (CLUSTER == 1 && (BN == 64 || BN == 128)), "FP8: two accumulator sets fit at BN <= 128");
+  static_assert(EPI == kEpiGeneral || (!FP8 && CLUSTER == 1 && BN >= 128), "epilogue kinds: fp16 BN 128 / 256 only");
+  static_assert(!TIMELINE || (!FP8 && CLUSTER == 1), "timeline: fp16 single-CTA kernels only");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -496,10 +649,21 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
     }
   };
+  // timeline (TIMELINE only): lane 0 of each warpgroup stores stamp k of a recorded tile as it takes it, and the slot is
+  // derived from the tile index, so that the timeline holds no register across the tile (the 256-wide kinds have none)
+  auto stamp = [&](const TileIter& it, int k) {
+    if (TIMELINE && p.timeline != nullptr && (threadIdx.x & 127) == 0) {
+      const int slot = (it.tile - tile0) / tile_step;
+      if (slot < p.timeline_slots)
+        p.timeline[((static_cast<size_t>(blockIdx.x) * p.timeline_slots + slot) * 2 + wg) * 4 + k] = globaltimer();
+    }
+  };
+  if (TIMELINE && p.timeline != nullptr && threadIdx.x == 0) p.timeline_sm[blockIdx.x] = static_cast<int>(smid());
   for (TileIter it(tiles_m, tiles_n, m_stationary, p.m_fast != 0, tile0, tile_step); it.valid(); it.next()) {
     const int m0 = it.m0(kRows) + rank * kGemmBM;
     const int n0 = it.n0(BN);
     int prev = -1;
+    if constexpr (TIMELINE) stamp(it, 0);
     if constexpr (FP8) {
       // per k-block: four k32 MMAs into a fresh tile, then the promotion  acc += tile * (s_a[row] * s_w).  The tile is
       // reused by the next k-block, so each warpgroup waits for its MMAs; the other warpgroup's keep the tensor core busy.
@@ -531,6 +695,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     } else {
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
+        if constexpr (TIMELINE) if (kb == 0) stamp(it, 1);
         const uint32_t sa = smem_base + stage * S::kStageBytes + wg * (64 * 128);
         const uint32_t sb = smem_base + stage * S::kStageBytes + S::kABytes;
         wgmma_fence_operand(acc);
@@ -549,6 +714,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       }
       wgmma_wait<0>();
       wgmma_fence_operand(acc);
+      if constexpr (TIMELINE) stamp(it, 2);
       if (prev >= 0) release(prev);
     }
 
@@ -618,9 +784,12 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       const uint32_t row_inv = smem_base + S::kRowScaleOffset + wg * 64 * 4;
       if (p.out8) gemm_row_scales_e4m3<BN>(p, acc, m0, n0, r0, c0, wg, M_eff, row_inv);
       gemm_epilogue_rows<BN, true>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16, row_inv);
+    } else if constexpr (EPI != kEpiGeneral) {
+      gemm_epilogue_kind<BN, EPI>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
     } else {
       gemm_epilogue_rows<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16);
     }
+    if constexpr (TIMELINE) stamp(it, 3);
   }
   // the peer may still arrive on this CTA's barriers: neither CTA leaves before both are done
   if constexpr (CLUSTER == 2) cluster_sync_all();

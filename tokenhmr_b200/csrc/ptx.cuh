@@ -40,6 +40,17 @@ __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ uint32_t smid() {
+  uint32_t s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+
 __device__ __forceinline__ uint32_t lane_id() {
   uint32_t l;
   asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
