@@ -6,7 +6,8 @@ general one, and prints one JSON line per case:
   (a) CUDA-event time per launch over 40 launches after warm-up, at the full K and at K = 64 (one k-block per tile,
       so almost only the fixed per-tile cost is left);
   (b) median, p90 and mean of each phase per tile from the kernel's %globaltimer timeline (GemmParams::timeline):
-      wait = tile start -> first full barrier, mma = -> last wgmma retired, epilogue = -> epilogue done;
+      wait = tile start -> first full barrier, mma = -> last wgmma retired, epilogue = -> epilogue done (for the
+      TMA-stored fp16 kinds: the tile's stores issued, not completed);
   (c) torch.matmul fp16 at the same M, N, K, with no epilogue, as the card's own yardstick for these shapes;
   (d) card name, power limit and SM clocks, read in the same run.
 

@@ -8,6 +8,7 @@ namespace thmr {
 
 struct GemmPlan {
   CUtensorMap tmA, tmB;
+  CUtensorMap tmC;   // out16, box 64 x 64, SWIZZLE_128B: the TMA stores of the fp16 kinds (zero for the other plans)
   GemmParams p;
   int bn;
   int grid;
@@ -49,13 +50,13 @@ struct GemmDesc {
 // 128 * BN * 64 MACs), so they win unless they leave SMs idle or their epilogue dominates.  Cost model per tile in
 // cycles on an H100 SM: per k-block max(MMA at 2048 fp16 MAC/clk, operand feed at ~32 B/clk from L2) plus a fixed
 // overhead, plus the epilogue.  The epilogue terms are fitted to the ViT GEMMs (M = 12288) on an H100 80GB HBM3 (700 W
-// power limit; scripts/gemm_anatomy.py, per-tile timeline at K = 64), so that the model picks the measured-faster width
-// at all five of them.  The specialised epilogue kinds (fast_epilogue, block_n 128 / 256 only) cost 2.3-3.6 us per
-// 128 x 128 tile and 4-8 us per 128 x 256 tile (fp16 outputs; the fp32 residual ones move twice the bytes), ~5000
-// cycles per 128 columns, so 256 wins at all five.  The general epilogue costs ~30 us per 128 x 256 tile (eight
+// power limit; scripts/gemm_anatomy.py, per-tile timeline), so that the model picks the measured-faster width at all
+// five of them.  Of the specialised epilogue kinds (block_n 128 / 256 only), the TMA-stored fp16 ones hold the
+// consumers 0.8-2.3 us per 128 columns (~2500 cycles), the fp32 residual one ~7 us (~12000 cycles: it reads and writes
+// 8 bytes per element); 256 wins at all five either way.  The general epilogue costs ~30 us per 128 x 256 tile (eight
 // 32-column chunks) against ~7 us per 128 x 128 tile; the narrower tiles are scaled from 128.  The row arg-min
 // epilogue (VQ) is not staged and is not charged.
-inline int pick_bn(int M, int N, int K, bool staged_epilogue, bool fast_epilogue, int force) {
+inline int pick_bn(int M, int N, int K, bool staged_epilogue, int epi_kind, int force) {
   if (force) return force;
   const int sms = num_sms();
   const int tm = (M + kGemmBM - 1) / kGemmBM;
@@ -69,10 +70,11 @@ inline int pick_bn(int M, int N, int K, bool staged_epilogue, bool fast_epilogue
     const long waves = (tiles + sms - 1) / sms;
     const double mma = 4.0 * bn;
     const double feed = (128.0 + bn) * 128.0 / 32.0;
-    const double epilogue = !staged_epilogue                 ? 0.0
-                            : fast_epilogue && bn >= 128      ? 5000.0 * bn / 128
-                            : bn == 256                       ? 55000.0
-                                                              : 7000.0 * bn / 128;
+    const double epilogue = !staged_epilogue                                 ? 0.0
+                            : bn >= 128 && gemm_epi_tma_store(epi_kind)       ? 2500.0 * bn / 128
+                            : bn >= 128 && epi_kind == kEpiBiasResidF32       ? 12000.0 * bn / 128
+                            : bn == 256                                       ? 55000.0
+                                                                              : 7000.0 * bn / 128;
     const double cost = waves * (num_kb * ((mma > feed ? mma : feed) + 40.0) + epilogue);
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = bn; }
   }
@@ -150,6 +152,7 @@ inline int gemm_make_plan_fp8(const GemmDesc& d, GemmPlan* plan) {
   p.out8 = d.out8; p.ld8 = d.ld8; p.out8_scale = d.out8_scale; p.ld8s = d.ld8s;
   THMR_TRY(make_tmap_2d_e4m3(&plan->tmA, d.A, d.a_rows, d.K, d.lda, kGemmBM, 128));
   THMR_TRY(make_tmap_2d_e4m3(&plan->tmB, d.B, d.N, d.K, d.ldb, bn, 128));
+  memset(&plan->tmC, 0, sizeof(plan->tmC));
   THMR_CHECK(d.force_epi == 0 || d.force_epi == 1 + kEpiGeneral, "gemm fp8: general epilogue only");
   plan->bn = bn;
   plan->cluster = 1;
@@ -169,8 +172,8 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   THMR_CHECK(d.out32 || d.out16 || d.argmin_out, "gemm: no output");
   const int cluster = d.force_bn == 512 ? 2 : 1;
   THMR_CHECK(cluster == 1 || !d.argmin_out, "gemm: block_n 512 (CTA pair) does not support the arg-min modes");
-  const bool fast_epi = gemm_pick_epi(d, 256, cluster) != kEpiGeneral;   // the kind does not depend on the width
-  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.K, d.argmin_out == nullptr, fast_epi, d.force_bn);
+  const int kind = gemm_pick_epi(d, 256, cluster);   // the kind does not depend on the width
+  const int bn = cluster == 2 ? 256 : pick_bn(d.M, d.N, d.K, d.argmin_out == nullptr, kind, d.force_bn);
   THMR_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: bad block_n %d", bn);
   GemmParams& p = plan->p;
   memset(&p, 0, sizeof(p));
@@ -205,6 +208,9 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
   THMR_CHECK(d.force_epi == 0 || d.force_epi - 1 == kEpiGeneral || d.force_epi - 1 == plan->epi,
              "gemm: epilogue kind %d does not fit this GEMM (its kind is %d)", d.force_epi - 1, plan->epi);
   if (d.force_epi) plan->epi = d.force_epi - 1;
+  memset(&plan->tmC, 0, sizeof(plan->tmC));
+  if (gemm_epi_tma_store(plan->epi))   // gemm_pick_epi checked the 16-byte base and pitch TMA needs
+    THMR_TRY(make_tmap_2d_f16(&plan->tmC, d.out16, d.M, d.N, d.ld16, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B));
   const long tiles_m = (d.M + kGemmBM * cluster - 1) / (kGemmBM * cluster);
   const long tiles = d.argmin_out ? tiles_m : tiles_m * ((d.N + bn - 1) / bn);
   // the CTAs of a wave should share tiles of the larger operand (TileIter)
@@ -236,7 +242,8 @@ inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8, EPI, TIMELINE>, plan.tmA, plan.tmB, plan.p));
+  THMR_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8, EPI, TIMELINE>, plan.tmA, plan.tmB,
+                               plan.tmC, plan.p));
   return THMR_OK;
 }
 

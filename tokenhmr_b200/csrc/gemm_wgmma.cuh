@@ -17,8 +17,10 @@
 // The producer runs ahead into the next tile while the consumers store the current one, so the epilogue overlaps the
 // operand loads of the next tile.  The element-wise epilogue stages the accumulators through shared memory and stores
 // whole row segments (gemm_epilogue_rows); it handles alpha scale, bias, a residual (may alias out32: same element,
-// same thread), residual tables, padded-sequence masking, activations, fp32 and / or fp16 outputs.  The row-argmin
-// modes of the VQ nearest-code search work straight from the accumulator registers.
+// same thread), residual tables, padded-sequence masking, activations, fp32 and / or fp16 outputs.  The fp16-output
+// epilogue kinds instead hand their finished tiles to TMA stores and go straight on to the next tile
+// (gemm_epilogue_f16_tma).  The row-argmin modes of the VQ nearest-code search work straight from the accumulator
+// registers.
 //
 // The same kernel runs the implicit-GEMM Conv1d (k=3, dilated) of the pose-token decoder: k-blocks are
 // grouped in "taps", each tap reads the A rows shifted by a row offset (TMA zero-fills out-of-range rows).
@@ -31,12 +33,15 @@ namespace thmr {
 enum : int { kActNone = 0, kActGelu = 1, kActRelu = 2 };
 
 // Epilogue kinds (GemmPlan::epi, a template parameter of the kernel).  kEpiGeneral (gemm_epilogue_rows) compiles every
-// option of GemmParams in; the others compile only what the ViT's call sites use (gemm_epilogue_kind):
-//   kEpiF16           alpha * acc -> fp16                          decoder to_kv
-//   kEpiBiasF16       alpha * acc + bias -> fp16                   QKV
-//   kEpiBiasGeluF16   GELU(alpha * acc + bias) -> fp16             fc1
-//   kEpiBiasResidF32  alpha * acc + bias + resid -> fp32           proj, fc2 (resid aliases out32)
+// option of GemmParams in; the others compile only what the ViT's call sites use:
+//   kEpiF16           alpha * acc -> fp16                          decoder to_kv   (gemm_epilogue_f16_tma)
+//   kEpiBiasF16       alpha * acc + bias -> fp16                   QKV             (gemm_epilogue_f16_tma)
+//   kEpiBiasGeluF16   GELU(alpha * acc + bias) -> fp16             fc1             (gemm_epilogue_f16_tma)
+//   kEpiBiasResidF32  alpha * acc + bias + resid -> fp32           proj, fc2 (resid aliases out32; gemm_epilogue_resid)
 enum : int { kEpiGeneral = 0, kEpiF16 = 1, kEpiBiasF16 = 2, kEpiBiasGeluF16 = 3, kEpiBiasResidF32 = 4 };
+
+// The fp16-output kinds store their tiles with TMA through GemmPlan::tmC.
+constexpr bool gemm_epi_tma_store(int epi) { return epi == kEpiF16 || epi == kEpiBiasF16 || epi == kEpiBiasGeluF16; }
 
 struct GemmParams {
   int M, N, K;
@@ -91,7 +96,8 @@ struct GemmParams {
   int ld8s;
   // per-tile phase timeline (gemm_f16_tn_kernel<..., TIMELINE = true>, test probe only): lane 0 of each consumer
   // warpgroup writes four %globaltimer stamps per tile into timeline[cta][slot][wg][4] (tile start, first full barrier
-  // passed, last wgmma retired, epilogue done) for the CTA's first timeline_slots tiles, and %smid into timeline_sm[cta]
+  // passed, last wgmma retired, epilogue done -- for the TMA-stored fp16 kinds: the tile's stores issued, not completed)
+  // for the CTA's first timeline_slots tiles, and %smid into timeline_sm[cta]
   unsigned long long* timeline;
   int timeline_slots;
   int* timeline_sm;
@@ -146,13 +152,17 @@ struct GemmSmem {
   static constexpr uint32_t kABytes = kGemmBM * kGemmBK * 2;
   static constexpr uint32_t kBBytes = BN * kGemmBK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;   // multiple of 1024: every operand tile stays swizzle-aligned
+  // epilogue staging, 16 KB per warpgroup: a 64 x gemm_chunk block of fp32 accumulators (general and residual
+  // epilogues) or a 64 x 128 fp16 output tile, two 128B-swizzled TMA store boxes (fp16 kinds), so 1024-byte aligned
+  static constexpr uint32_t kEpiOffset = STAGES * kStageBytes;
+  static constexpr uint32_t kEpiWgBytes = 64 * 128 * 2;
+  static_assert(64 * gemm_chunk<BN>() * 4 <= kEpiWgBytes, "fp32 staging chunk exceeds the warpgroup's block");
+  static constexpr uint32_t kEpiBytes = 2 * kEpiWgBytes;
   // FP8: the 128 activation scales of each stage's k-block ride the same ring, outside the swizzled operand tiles
-  static constexpr uint32_t kScaleOffset = STAGES * kStageBytes;
+  static constexpr uint32_t kScaleOffset = kEpiOffset + kEpiBytes;
   static constexpr uint32_t kScaleBytes = FP8 ? STAGES * kGemmBM * 4 : 0;
   static constexpr uint32_t kBarOffset = kScaleOffset + kScaleBytes;
-  static constexpr uint32_t kEpiOffset = kBarOffset + 256;     // epilogue staging, one 64 x chunk block per warpgroup
-  static constexpr uint32_t kEpiBytes = 2 * 64 * gemm_chunk<BN>() * 4;
-  static constexpr uint32_t kRowScaleOffset = kEpiOffset + kEpiBytes;   // FP8 e4m3 output: 1 / scale of each tile row
+  static constexpr uint32_t kRowScaleOffset = kBarOffset + 256;   // FP8 e4m3 output: 1 / scale of each tile row
   static constexpr uint32_t kRowScaleBytes = FP8 ? kGemmBM * 4 : 0;
   static constexpr uint32_t kTotal = kRowScaleOffset + kRowScaleBytes + 1024;  // alignment slack
 };
@@ -376,34 +386,25 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
   }
 }
 
-// The octet of a partial column tile (col < N < col + 8) of gemm_epilogue_kind, element by element.
-template <int EPI>
-__device__ __forceinline__ void gemm_epilogue_kind_tail(const GemmParams& p, const float (&v)[8], int row, int col) {
+// The octet of a partial column tile (col < N < col + 8) of gemm_epilogue_resid, element by element.
+__device__ __forceinline__ void gemm_epilogue_resid_tail(const GemmParams& p, const float (&v)[8], int row, int col) {
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     if (col + e >= p.N) break;
-    float x = __fmul_rn(v[e], p.alpha);
-    if constexpr (EPI != kEpiF16) x = __fadd_rn(x, __ldg(p.bias + col + e));
-    if constexpr (EPI == kEpiBiasResidF32) {
-      const size_t i = static_cast<size_t>(row) * p.ld32 + col + e;
-      p.out32[i] = __fadd_rn(x, p.resid[static_cast<size_t>(row) * p.ldr + col + e]);
-    } else {
-      if constexpr (EPI == kEpiBiasGeluF16) x = gelu_erf(x);
-      p.out16[static_cast<size_t>(row) * p.ld16 + col + e] = __float2half_rn(x);
-    }
+    const float x = __fadd_rn(__fmul_rn(v[e], p.alpha), __ldg(p.bias + col + e));
+    const float r = p.resid[static_cast<size_t>(row) * p.ldr + col + e];
+    p.out32[static_cast<size_t>(row) * p.ld32 + col + e] = __fadd_rn(x, r);
   }
 }
 
-// Element-wise epilogue of one consumer warpgroup for a specialised kind (kEpiF16 .. kEpiBiasResidF32): the staging
-// and the row walk of gemm_epilogue_rows and the same values element for element, but only the kind's operations are
-// compiled, and the chunks go through one rolled loop, so that the walk is emitted once instead of once per chunk.
-// Only the fragment staging is unrolled per chunk (a uniform branch picks it), since it indexes registers.  The plan
-// (gemm_make_plan) guarantees 16-byte aligned bases and pitches for every operand the kind touches.
-template <int BN, int EPI>
-__device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
-                                                   int m0w, int n0, int M_eff, uint32_t bar_id) {
-  constexpr bool kBias = EPI != kEpiF16;
-  constexpr bool kResid = EPI == kEpiBiasResidF32;
+// Element-wise epilogue of one consumer warpgroup for kEpiBiasResidF32: the staging and the row walk of
+// gemm_epilogue_rows and the same values element for element, but only the kind's operations are compiled, and the
+// chunks go through one rolled loop, so that the walk is emitted once instead of once per chunk.  Only the fragment
+// staging is unrolled per chunk (a uniform branch picks it), since it indexes registers.  The plan (gemm_make_plan)
+// guarantees 16-byte aligned bases and pitches for the bias, the residual and out32.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue_resid(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
+                                                    int m0w, int n0, int M_eff, uint32_t bar_id) {
   constexpr int CH = gemm_chunk<BN>();
   constexpr int OCT = CH / 8;
   constexpr int ITEMS = OCT / 2;
@@ -423,7 +424,7 @@ __device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const fl
     const int ccol = n0 + c * CH + 8 * (lane >> 3);
     float bias[ITEMS / 2][8];
     float res[ITEMS][8];
-    if constexpr (kBias && !(kResid && ITEMS == 2)) {
+    if constexpr (ITEMS != 2) {
 #pragma unroll
       for (int ob = 0; ob < ITEMS / 2; ++ob) {
         const int col = ccol + 32 * ob;
@@ -435,19 +436,17 @@ __device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const fl
         }
       }
     }
-    if constexpr (kResid) {
-      // all residual loads of the chunk before any of its stores
+    // all residual loads of the chunk before any of its stores
 #pragma unroll
-      for (int k = 0; k < ITEMS; ++k) {
-        const int row = m0w + 8 * (w4 + 4 * (k & 1)) + (lane & 7);
-        const int col = ccol + 32 * (k >> 1);
-        if (row < M_eff && col + 8 <= p.N) {
-          const float* r = p.resid + static_cast<size_t>(row) * p.ldr + col;
-          const float4 x0 = *reinterpret_cast<const float4*>(r);
-          const float4 x1 = *reinterpret_cast<const float4*>(r + 4);
-          res[k][0] = x0.x; res[k][1] = x0.y; res[k][2] = x0.z; res[k][3] = x0.w;
-          res[k][4] = x1.x; res[k][5] = x1.y; res[k][6] = x1.z; res[k][7] = x1.w;
-        }
+    for (int k = 0; k < ITEMS; ++k) {
+      const int row = m0w + 8 * (w4 + 4 * (k & 1)) + (lane & 7);
+      const int col = ccol + 32 * (k >> 1);
+      if (row < M_eff && col + 8 <= p.N) {
+        const float* r = p.resid + static_cast<size_t>(row) * p.ldr + col;
+        const float4 x0 = *reinterpret_cast<const float4*>(r);
+        const float4 x1 = *reinterpret_cast<const float4*>(r + 4);
+        res[k][0] = x0.x; res[k][1] = x0.y; res[k][2] = x0.z; res[k][3] = x0.w;
+        res[k][4] = x1.x; res[k][5] = x1.y; res[k][6] = x1.z; res[k][7] = x1.w;
       }
     }
 #pragma unroll
@@ -465,10 +464,10 @@ __device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const fl
         v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
       }
       if (col + 8 > p.N) {
-        gemm_epilogue_kind_tail<EPI>(p, v, row, col);
+        gemm_epilogue_resid_tail(p, v, row, col);
         continue;
       }
-      if constexpr (kResid && ITEMS == 2) {
+      if constexpr (ITEMS == 2) {
         // 128 accumulators stay live across the rolled chunk loop: the 32-column chunks of BN = 256 have no registers
         // left to hold the bias from before the residual loads, so it is read here
         const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
@@ -477,26 +476,74 @@ __device__ __forceinline__ void gemm_epilogue_kind(const GemmParams& p, const fl
         bias[0][4] = b1.x; bias[0][5] = b1.y; bias[0][6] = b1.z; bias[0][7] = b1.w;
       }
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        v[e] = __fmul_rn(v[e], p.alpha);
-        if constexpr (kBias) v[e] = __fadd_rn(v[e], bias[k >> 1][e]);
-        if constexpr (kResid) v[e] = __fadd_rn(v[e], res[k][e]);
-        if constexpr (EPI == kEpiBiasGeluF16) v[e] = gelu_erf(v[e]);
-      }
-      if constexpr (kResid) {
-        float4* o = reinterpret_cast<float4*>(p.out32 + static_cast<size_t>(row) * p.ld32 + col);
-        o[0] = make_float4(v[0], v[1], v[2], v[3]);
-        o[1] = make_float4(v[4], v[5], v[6], v[7]);
-      } else {
-        uint4 q;
-        __half2* h2 = reinterpret_cast<__half2*>(&q);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) h2[e] = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
-        *reinterpret_cast<uint4*>(p.out16 + static_cast<size_t>(row) * p.ld16 + col) = q;
-      }
+      for (int e = 0; e < 8; ++e)
+        v[e] = __fadd_rn(__fadd_rn(__fmul_rn(v[e], p.alpha), bias[k >> 1][e]), res[k][e]);
+      float4* o = reinterpret_cast<float4*>(p.out32 + static_cast<size_t>(row) * p.ld32 + col);
+      o[0] = make_float4(v[0], v[1], v[2], v[3]);
+      o[1] = make_float4(v[4], v[5], v[6], v[7]);
     }
     // the next chunk (or tile) overwrites the staging block
     named_barrier_sync(bar_id, 128);
+  }
+}
+
+// Epilogue of one consumer warpgroup for the fp16-output kinds (kEpiF16, kEpiBiasF16, kEpiBiasGeluF16): its 64 rows x
+// BN columns, rows m0w.. of the output.  The values are computed in the accumulator fragment with the rounding steps of
+// gemm_epilogue_rows (so they equal the general epilogue's bit for bit), rounded to fp16 and written into the
+// warpgroup's staging tile of 64 rows x 128 columns: two 64 x 64 boxes of out16's tensor map (GemmPlan::tmC), each in
+// the SWIZZLE_128B layout (row r: 128 bytes, 16-byte unit u at u ^ (r % 8)), so the fragment writes (eight rows of one
+// unit per warp store) are free of bank conflicts.  One thread then issues the TMA stores and the warpgroup goes on to
+// the next tile without waiting for them; TMA clips the boxes at [M, N], so partial tiles need no scalar tail.  BN = 256
+// takes two passes through the staging tile.  Before the tile is overwritten, the issuing thread waits until the
+// previous stores have read it.
+template <int BN, int EPI>
+__device__ __forceinline__ void gemm_epilogue_f16_tma(const GemmParams& p, const float (&acc)[BN / 2],
+                                                      const CUtensorMap* tm, uint32_t stage, int m0w, int n0,
+                                                      int M_eff, uint32_t bar_id) {
+  static_assert(gemm_epi_tma_store(EPI) && BN % 128 == 0, "fp16 TMA-store kinds, 128-column passes");
+  const int lane = threadIdx.x & 31;
+  const bool issuer = (threadIdx.x & 127) == 0;
+  // fragment: rows fr, fr + 8 of the warpgroup (both = lane / 4 mod 8), columns 8 j + c0 + {0, 1}
+  const int fr = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const int swz = lane >> 2;
+#pragma unroll
+  for (int q = 0; q < BN / 128; ++q) {
+    const int nq = n0 + 128 * q;
+    if (nq >= p.N) break;
+    if (issuer) tma_store_wait_read<0>();
+    named_barrier_sync(bar_id, 128);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = nq + 8 * j + c0;
+      float b[2] = {0.f, 0.f};
+      if constexpr (EPI != kEpiF16) {
+        // columns past N are clipped by the store, so their bias may be any value
+        b[0] = __ldg(p.bias + min(col, p.N - 1));
+        b[1] = __ldg(p.bias + min(col + 1, p.N - 1));
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float v[2];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          v[c] = __fmul_rn(acc[64 * q + 4 * j + 2 * i + c], p.alpha);
+          if constexpr (EPI != kEpiF16) v[c] = __fadd_rn(v[c], b[c]);
+          if constexpr (EPI == kEpiBiasGeluF16) v[c] = gelu_erf(v[c]);
+        }
+        const __half2 h = __floats2half2_rn(v[0], v[1]);
+        sts_u32(stage + (j >> 3) * 8192 + (fr + 8 * i) * 128 + (((j & 7) ^ swz) << 4) + 2 * c0,
+                *reinterpret_cast<const uint32_t*>(&h));
+      }
+    }
+    // the staging writes become visible to the TMA unit (async proxy) before it reads them
+    fence_proxy_async_smem();
+    named_barrier_sync(bar_id, 128);
+    if (issuer && m0w < M_eff) {
+      tma_store_2d(tm, stage, nq, m0w);
+      if (nq + 64 < p.N) tma_store_2d(tm, stage + 8192, nq + 64, m0w);
+      tma_store_commit();
+    }
   }
 }
 
@@ -535,7 +582,8 @@ __device__ __forceinline__ void gemm_row_scales_e4m3(const GemmParams& p, float 
 
 template <int BN, int STAGES, int CLUSTER, bool FP8 = false, int EPI = kEpiGeneral, bool TIMELINE = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   using S = GemmSmem<BN, STAGES, FP8>;
   constexpr int BK = gemm_bk<FP8>();
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
@@ -578,6 +626,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   if (warp == kWarpTma && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (gemm_epi_tma_store(EPI)) tma_prefetch_desc(&tmC);
   }
   if constexpr (CLUSTER == 2) cluster_sync_all();   // the peer's barriers are initialised before any multicast or arrive
   else __syncthreads();
@@ -624,7 +673,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const bool vec_r = p.resid && p.ldr % 4 == 0 && aligned16(p.resid);
   const bool vec32 = p.out32 && p.ld32 % 4 == 0 && aligned16(p.out32);
   const bool vec16 = p.out16 && p.ld16 % 8 == 0 && aligned16(p.out16);
-  const uint32_t epi_stage = smem_base + S::kEpiOffset + wg * 64 * gemm_chunk<BN>() * 4;
+  const uint32_t epi_stage = smem_base + S::kEpiOffset + wg * S::kEpiWgBytes;
   const bool screen = p.argmin_out != nullptr && p.screen_rows != nullptr;
   const float m2a = -2.0f * p.alpha;
   // accumulator fragment of this thread: rows r0, r0 + 8 of the tile, columns 8 j + c0 + {0, 1}
@@ -784,13 +833,18 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       const uint32_t row_inv = smem_base + S::kRowScaleOffset + wg * 64 * 4;
       if (p.out8) gemm_row_scales_e4m3<BN>(p, acc, m0, n0, r0, c0, wg, M_eff, row_inv);
       gemm_epilogue_rows<BN, true>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16, row_inv);
+    } else if constexpr (EPI == kEpiBiasResidF32) {
+      gemm_epilogue_resid<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
     } else if constexpr (EPI != kEpiGeneral) {
-      gemm_epilogue_kind<BN, EPI>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
+      gemm_epilogue_f16_tma<BN, EPI>(p, acc, &tmC, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
     } else {
       gemm_epilogue_rows<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16);
     }
     if constexpr (TIMELINE) stamp(it, 3);
   }
+  // the last tile's TMA stores complete (and stop reading the staging tile) before the CTA exits
+  if constexpr (gemm_epi_tma_store(EPI))
+    if ((threadIdx.x & 127) == 0) tma_store_wait<0>();
   // the peer may still arrive on this CTA's barriers: neither CTA leaves before both are done
   if constexpr (CLUSTER == 2) cluster_sync_all();
 }

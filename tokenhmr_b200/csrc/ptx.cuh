@@ -30,6 +30,7 @@ __device__ __forceinline__ float4 lds_f32x4(uint32_t a) {
   return v;
 }
 __device__ __forceinline__ void sts_f32(uint32_t a, float x) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(x)); }
+__device__ __forceinline__ void sts_u32(uint32_t a, uint32_t x) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(x)); }
 __device__ __forceinline__ float lds_f32(uint32_t a) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
@@ -165,11 +166,12 @@ __device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const CUtensor
         "h"(cta_mask)
       : "memory");
 }
-// 2D tiled store shared -> global (bulk group completion).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
+// 2D tiled store shared (32-bit shared address) -> global (bulk group completion); the box is clipped at the tensor's
+// bounds.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                :
-               : "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
