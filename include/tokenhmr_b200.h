@@ -40,7 +40,8 @@ typedef enum thmr_status {
 
 int thmr_abi_version(void);
 const char* thmr_last_error(void);
-/* Reads and clears the device-side pipeline-timeout flag (synchronises the device). */
+/* Reads and clears the device-side flags (synchronises the device): a pipeline timeout, a strict-mode range overflow,
+ * and an unsupported smpl_params_is_axis_angle given to thmr_tokenhmr_loss. */
 int thmr_check_device_flags(void);
 
 /* ================================================================================================
@@ -225,6 +226,62 @@ typedef struct thmr_smplify_desc {
 } thmr_smplify_desc;
 size_t thmr_smplify_workspace_bytes(const thmr_smpl* m, int B, int num_iters);
 int thmr_smplify_inv(const thmr_smpl* m, const thmr_smplify_desc* desc, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Training loss: TokenHMR.compute_loss [tokenhmr/lib/models/tokenhmr.py:190-277 with losses.py] and the camera tail of
+ * forward_step [tokenhmr.py:162-187] with its backward (DESIGN §2 "Training loss")
+ * ---------------------------------------------------------------------------------------------- */
+/* The camera tail alone: joints fp32 [B,J,3], pred_cam [B,3] (s, tx, ty) -> cam_t [B,3] = (tx, ty, 2 focal /
+ * (image_size s + 1e-9)), focal_out [B,2] (nullable), kp2d [B,J,2] = (focal / image_size) (X + t)_xy / (X + t)_z.
+ * Bitwise the numbers thmr_smpl_forward's fused tail writes for the same joints and camera. */
+int thmr_camera_tail(const float* joints, const float* pred_cam, int B, int J, float focal_length, float image_size,
+                     float* cam_t, float* focal_out, float* kp2d, void* stream);
+/* Its VJP: grad_kp2d [B,J,2] and grad_cam_t [B,3] are nullable (null = zero cotangent); writes grad_joints [B,J,3] and
+ * grad_pred_cam [B,3].  Recomputes the forward from joints and pred_cam. */
+int thmr_camera_tail_backward(const float* joints, const float* pred_cam, int B, int J, float focal_length,
+                              float image_size, const float* grad_kp2d, const float* grad_cam_t, float* grad_joints,
+                              float* grad_pred_cam, void* stream);
+
+/* One loss evaluation, and optionally its gradient, in two kernels.  tals = 1 is the threshold-adaptive branch
+ * (cfg.MODEL.LOOSE_SUP and train: tokenhmr.py:214-249), which needs num_joints == 44 (the size of losses.py's
+ * kp2D_err_valid_thresh); tals = 0 is the plain branch (:250-262).  The GT axis-angles go through geometry.aa_to_rotmat,
+ * and every mask decision is taken in double.  Reductions are sums over the batch in a fixed order; the call does no
+ * host synchronisation and no allocation (graph-capturable) and never writes an input.  The smpl_params_is_axis_angle
+ * flags must be (1, 1, 0) for every sample, as the reference's loaders emit them; otherwise a device flag is raised and
+ * thmr_check_device_flags returns THMR_ERR_INVALID.  All pointers are device pointers, fp32 unless noted. */
+typedef struct thmr_loss_desc {
+  int B;                          /* >= 1 */
+  int num_joints;                 /* J */
+  int num_betas;                  /* 1 .. 10 */
+  int tals;                       /* 1: LOOSE_SUP and train;  0: plain (validation, or LOOSE_SUP false) */
+  int pelvis_id;                  /* 0 .. J-1: the 3-D keypoints are aligned at this joint (25 + 14) */
+  double loose_weight;            /* cfg.MODEL.LOOSE_WEIGHT */
+  double w_keypoints_2d, w_keypoints_3d, w_global_orient, w_body_pose, w_betas;   /* cfg.LOSS_WEIGHTS */
+  const float* pred_keypoints_2d; /* [B,J,2] */
+  const float* pred_keypoints_3d; /* [B,J,3] */
+  const float* pred_rotmats;      /* [B,24,3,3]: global_orient, then body_pose */
+  const float* pred_betas;        /* [B,num_betas] */
+  const float* gt_keypoints_2d;   /* [B,J,3] with confidence */
+  const float* gt_keypoints_3d;   /* [B,J,4] with confidence */
+  const float* gt_global_orient;  /* [B,3] axis-angle */
+  const float* gt_body_pose;      /* [B,69] axis-angle */
+  const float* gt_betas;          /* [B,num_betas] */
+  const float* has_global_orient; /* [B] has_smpl_params */
+  const float* has_body_pose;     /* [B] */
+  const float* has_betas;         /* [B] */
+  const float* valid_3d;          /* [B] 1 for an H36M-TRAIN-WMASK or BEDLAM sample, else 0 (read when tals = 1) */
+  const uint8_t* is_axis_angle_global_orient; /* [B] bool smpl_params_is_axis_angle */
+  const uint8_t* is_axis_angle_body_pose;     /* [B] */
+  const uint8_t* is_axis_angle_betas;         /* [B] */
+  float* losses;                  /* [6] loss, keypoints_2d, keypoints_3d, global_orient, body_pose, betas */
+  /* d loss / d input for a unit upstream gradient; all four set or all four NULL */
+  float* grad_keypoints_2d;       /* [B,J,2] */
+  float* grad_keypoints_3d;       /* [B,J,3] */
+  float* grad_rotmats;            /* [B,24,3,3] */
+  float* grad_betas;              /* [B,num_betas] */
+} thmr_loss_desc;
+size_t thmr_tokenhmr_loss_workspace_bytes(int B);
+int thmr_tokenhmr_loss(const thmr_loss_desc* desc, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Tokenizer encoder + hard quantisation (SURVEY §8 row f4): EncodeTokens

@@ -34,6 +34,19 @@ class SmplifyDesc(Structure):
                 ("history", c_void_p), ("iters_run", c_void_p)]
 
 
+class LossDesc(Structure):
+    _fields_ = [("B", c_int), ("num_joints", c_int), ("num_betas", c_int), ("tals", c_int), ("pelvis_id", c_int),
+                ("loose_weight", ctypes.c_double), ("w_keypoints_2d", ctypes.c_double),
+                ("w_keypoints_3d", ctypes.c_double), ("w_global_orient", ctypes.c_double),
+                ("w_body_pose", ctypes.c_double), ("w_betas", ctypes.c_double)] + \
+               [(n, c_void_p) for n in ("pred_keypoints_2d", "pred_keypoints_3d", "pred_rotmats", "pred_betas",
+                                        "gt_keypoints_2d", "gt_keypoints_3d", "gt_global_orient", "gt_body_pose",
+                                        "gt_betas", "has_global_orient", "has_body_pose", "has_betas", "valid_3d",
+                                        "is_axis_angle_global_orient", "is_axis_angle_body_pose",
+                                        "is_axis_angle_betas", "losses", "grad_keypoints_2d", "grad_keypoints_3d",
+                                        "grad_rotmats", "grad_betas")]
+
+
 class Config(Structure):
     _fields_ = [("image_size", c_int), ("crop_w", c_int), ("patch", c_int), ("patch_pad", c_int),
                 ("vit_dim", c_int), ("vit_depth", c_int), ("vit_heads", c_int), ("vit_mlp_ratio", c_int),
@@ -207,6 +220,12 @@ SIGNATURES = {
                                   c_void_p, c_void_p]),
     "thmr_smplify_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int]),
     "thmr_smplify_inv": (c_int, [c_void_p, POINTER(SmplifyDesc), c_void_p, c_void_p]),
+    "thmr_camera_tail": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
+    "thmr_camera_tail_backward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_void_p]),
+    "thmr_tokenhmr_loss_workspace_bytes": (c_size_t, [c_int]),
+    "thmr_tokenhmr_loss": (c_int, [POINTER(LossDesc), c_void_p, c_void_p]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),
     "thmr_engine_workspace_bytes": (c_size_t, [c_void_p, c_int]),

@@ -282,6 +282,18 @@ smpl_skin_kernel(const int* __restrict__ w_idx, const float* __restrict__ w_val,
 }
 
 // ---- joints: 25 mapped + n_extra regressed, optional camera / projection --------------------------------
+// The camera tail of forward_step, shared with camera_tail_kernel (losses.cuh) so both give the same numbers.
+// tokenhmr.py:166-168: the depth of pred_cam_t from the scale s of pred_cam = (s, tx, ty)
+__device__ __forceinline__ float cam_depth(float s, float focal, float image_size) {
+  return 2.f * focal / (image_size * s + 1e-9f);
+}
+// perspective_projection with rotation I, camera centre 0, focal = focal/image_size (geometry.py:110-124)
+__device__ __forceinline__ float2 project_point(const float x[3], const float t[3], float focal, float image_size) {
+  const float px = x[0] + t[0], py = x[1] + t[1], pz = x[2] + t[2];
+  const float f = focal / image_size;
+  return make_float2(f * (px / pz), f * (py / pz));
+}
+
 __global__ void __launch_bounds__(64)
 smpl_joints_kernel(const float* __restrict__ Jposed, const float* __restrict__ verts, long vert_pitch,
                    const int* __restrict__ joint_map, const int* __restrict__ extra_vid,
@@ -297,7 +309,7 @@ smpl_joints_kernel(const float* __restrict__ Jposed, const float* __restrict__ v
     const float s = pred_cam[b * 3 + 0];
     t[0] = pred_cam[b * 3 + 1];
     t[1] = pred_cam[b * 3 + 2];
-    t[2] = 2.f * focal / (image_size * s + 1e-9f);          // tokenhmr.py:166-168
+    t[2] = cam_depth(s, focal, image_size);
     if (threadIdx.x == 0) {
       cam_t[b * 3 + 0] = t[0]; cam_t[b * 3 + 1] = t[1]; cam_t[b * 3 + 2] = t[2];
       focal_out[b * 2 + 0] = focal; focal_out[b * 2 + 1] = focal;
@@ -322,11 +334,9 @@ smpl_joints_kernel(const float* __restrict__ Jposed, const float* __restrict__ v
     float* o = joints + (static_cast<size_t>(b) * nj + k) * 3;
     o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
     if (pred_cam) {
-      // perspective_projection with rotation I, camera centre 0, focal = focal/image_size (geometry.py:110-124)
-      const float px = x[0] + t[0], py = x[1] + t[1], pz = x[2] + t[2];
-      const float f = focal / image_size;
-      kp2d[(static_cast<size_t>(b) * nj + k) * 2 + 0] = f * (px / pz);
-      kp2d[(static_cast<size_t>(b) * nj + k) * 2 + 1] = f * (py / pz);
+      const float2 u = project_point(x, t, focal, image_size);
+      kp2d[(static_cast<size_t>(b) * nj + k) * 2 + 0] = u.x;
+      kp2d[(static_cast<size_t>(b) * nj + k) * 2 + 1] = u.y;
     }
   }
 }

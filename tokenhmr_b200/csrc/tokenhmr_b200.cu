@@ -9,6 +9,7 @@
 #include "engine_strict.cuh"
 #include "eval_kernels.cuh"
 #include "keypoints.cuh"
+#include "losses.cuh"
 #include "preproc.cuh"
 #include "render.cuh"
 #include "smpl_grad.cuh"
@@ -60,6 +61,13 @@ int thmr_check_device_flags(void) {
     unsigned int zero = 0;
     THMR_CUDA(cudaMemcpyToSymbol(g_strict_overflow, &zero, sizeof(zero)));
     return fail(THMR_ERR_INVALID, "strict mode: an activation left the split-fp16 range (|a| >= 4094 or NaN)");
+  }
+  THMR_CUDA(cudaMemcpyFromSymbol(&flag, g_loss_flags, sizeof(flag)));
+  if (flag) {
+    unsigned int zero = 0;
+    THMR_CUDA(cudaMemcpyToSymbol(g_loss_flags, &zero, sizeof(zero)));
+    return fail(THMR_ERR_INVALID, "tokenhmr_loss: smpl_params_is_axis_angle must be (True, True, False) for "
+                                  "(global_orient, body_pose, betas) of every sample");
   }
   return THMR_OK;
 }
@@ -853,6 +861,52 @@ int thmr_smplify_inv(const thmr_smpl* s, const thmr_smplify_desc* d, void* works
   SmplifyWs ws;
   smplify_carve(bp, s->m, d->B, d->num_iters, &ws);
   return smplify_run(s, *d, ws, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------ training loss
+int thmr_camera_tail(const float* joints, const float* pred_cam, int B, int J, float focal_length, float image_size,
+                     float* cam_t, float* focal_out, float* kp2d, void* stream) {
+  THMR_CHECK(joints && pred_cam && cam_t && kp2d, "camera_tail: null argument");
+  THMR_CHECK(B > 0 && J > 0, "camera_tail: bad shape B=%d J=%d", B, J);
+  camera_tail_kernel<<<(B + kTailWarps - 1) / kTailWarps, 32 * kTailWarps, 0, static_cast<cudaStream_t>(stream)>>>(
+      joints, pred_cam, J, B, focal_length, image_size, cam_t, focal_out, kp2d);
+  THMR_CUDA(cudaGetLastError());
+  return THMR_OK;
+}
+
+int thmr_camera_tail_backward(const float* joints, const float* pred_cam, int B, int J, float focal_length,
+                              float image_size, const float* grad_kp2d, const float* grad_cam_t, float* grad_joints,
+                              float* grad_pred_cam, void* stream) {
+  THMR_CHECK(joints && pred_cam && grad_joints && grad_pred_cam, "camera_tail_backward: null argument");
+  THMR_CHECK(B > 0 && J > 0, "camera_tail_backward: bad shape B=%d J=%d", B, J);
+  camera_tail_backward_kernel<<<(B + kTailWarps - 1) / kTailWarps, 32 * kTailWarps, 0,
+                                static_cast<cudaStream_t>(stream)>>>(joints, pred_cam, J, B, focal_length, image_size,
+                                                                     grad_kp2d, grad_cam_t, grad_joints, grad_pred_cam);
+  THMR_CUDA(cudaGetLastError());
+  return THMR_OK;
+}
+
+size_t thmr_tokenhmr_loss_workspace_bytes(int B) { return B > 0 ? tokenhmr_loss_part_bytes(B) : 0; }
+
+int thmr_tokenhmr_loss(const thmr_loss_desc* d, void* workspace, void* stream) {
+  THMR_CHECK(d && workspace, "tokenhmr_loss: null desc or workspace");
+  THMR_CHECK(d->B >= 1 && d->num_joints >= 1, "tokenhmr_loss: B=%d J=%d", d->B, d->num_joints);
+  THMR_CHECK(d->num_betas >= 1 && d->num_betas <= 10, "tokenhmr_loss: num_betas %d (1 .. 10)", d->num_betas);
+  THMR_CHECK(d->tals == 0 || d->tals == 1, "tokenhmr_loss: tals %d (0 or 1)", d->tals);
+  THMR_CHECK(!d->tals || d->num_joints == kLossTalsJoints,
+             "tokenhmr_loss: the TALS branch needs %d keypoints (kp2D_err_valid_thresh), got %d", kLossTalsJoints,
+             d->num_joints);
+  THMR_CHECK(d->pelvis_id >= 0 && d->pelvis_id < d->num_joints, "tokenhmr_loss: pelvis_id %d outside [0, %d)",
+             d->pelvis_id, d->num_joints);
+  THMR_CHECK(d->pred_keypoints_2d && d->pred_keypoints_3d && d->pred_rotmats && d->pred_betas && d->gt_keypoints_2d &&
+                 d->gt_keypoints_3d && d->gt_global_orient && d->gt_body_pose && d->gt_betas && d->has_global_orient &&
+                 d->has_body_pose && d->has_betas && (d->valid_3d || !d->tals) && d->is_axis_angle_global_orient &&
+                 d->is_axis_angle_body_pose && d->is_axis_angle_betas && d->losses,
+             "tokenhmr_loss: missing input or output");
+  const int ng = (d->grad_keypoints_2d != nullptr) + (d->grad_keypoints_3d != nullptr) +
+                 (d->grad_rotmats != nullptr) + (d->grad_betas != nullptr);
+  THMR_CHECK(ng == 0 || ng == 4, "tokenhmr_loss: the four gradient outputs must be all set or all NULL");
+  return tokenhmr_loss_run(*d, workspace, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------ engine

@@ -318,6 +318,62 @@ def _wants_grad(*ts: torch.Tensor) -> bool:
     return torch.is_grad_enabled() and any(t.requires_grad for t in ts)
 
 
+# ------------------------------------------------------------------------------------------------ camera tail
+def camera_tail(joints: torch.Tensor, pred_cam: torch.Tensor, focal_length: float = 5000.0,
+                image_size: float = 256.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The camera tail of forward_step (tokenhmr.py:162-187): joints (B,J,3) and pred_cam (B,3) -> (pred_cam_t (B,3),
+    focal_length (B,2), keypoints_2d (B,J,2)), the numbers SMPLModel.forward(..., pred_cam=) gives for the same joints.
+    Differentiable in joints and pred_cam when grad mode is on and one of them requires grad
+    (thmr_camera_tail_backward)."""
+    if _wants_grad(joints, pred_cam):
+        return _CameraTailFn.apply(joints, pred_cam, float(focal_length), float(image_size))
+    return _camera_tail(joints, pred_cam, float(focal_length), float(image_size))
+
+
+def _camera_tail(joints: torch.Tensor, pred_cam: torch.Tensor, focal_length: float, image_size: float):
+    joints, pred_cam = _req(joints, torch.float32, "joints"), _req(pred_cam, torch.float32, "pred_cam")
+    if joints.dim() != 3 or joints.shape[2] != 3 or pred_cam.shape != (joints.shape[0], 3):
+        raise _lib.ThmrError(f"camera_tail: joints {tuple(joints.shape)} must be (B,J,3) and pred_cam "
+                             f"{tuple(pred_cam.shape)} (B,3)")
+    B, J = joints.shape[:2]
+    cam_t = torch.empty(B, 3, device=joints.device)
+    focal = torch.empty(B, 2, device=joints.device)
+    kp2d = torch.empty(B, J, 2, device=joints.device)
+    check(lib().thmr_camera_tail(joints.data_ptr(), pred_cam.data_ptr(), B, J, focal_length, image_size,
+                                 cam_t.data_ptr(), focal.data_ptr(), kp2d.data_ptr(), _stream()))
+    return cam_t, focal, kp2d
+
+
+class _CameraTailFn(torch.autograd.Function):
+    """camera_tail with thmr_camera_tail_backward as its backward (focal_length carries no gradient)."""
+
+    @staticmethod
+    def forward(ctx, joints: torch.Tensor, pred_cam: torch.Tensor, focal_length: float, image_size: float):
+        ctx.set_materialize_grads(False)
+        ctx.focal_length, ctx.image_size = focal_length, image_size
+        joints, pred_cam = joints.contiguous(), pred_cam.contiguous()
+        ctx.save_for_backward(joints, pred_cam)
+        cam_t, focal, kp2d = _camera_tail(joints, pred_cam, focal_length, image_size)
+        ctx.mark_non_differentiable(focal)
+        return cam_t, focal, kp2d
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_cam_t, _grad_focal, grad_kp2d):
+        joints, pred_cam = ctx.saved_tensors
+        if grad_cam_t is None and grad_kp2d is None:
+            return None, None, None, None
+        B, J = joints.shape[:2]
+        gk = None if grad_kp2d is None else _req(grad_kp2d, torch.float32, "grad_kp2d")
+        gc = None if grad_cam_t is None else _req(grad_cam_t, torch.float32, "grad_cam_t")
+        g_joints = torch.empty_like(joints)
+        g_cam = torch.empty_like(pred_cam)
+        check(lib().thmr_camera_tail_backward(joints.data_ptr(), pred_cam.data_ptr(), B, J, ctx.focal_length,
+                                              ctx.image_size, _ptr(gk), _ptr(gc), g_joints.data_ptr(),
+                                              g_cam.data_ptr(), _stream()))
+        return (g_joints if ctx.needs_input_grad[0] else None, g_cam if ctx.needs_input_grad[1] else None, None, None)
+
+
 class _SmplForwardFn(torch.autograd.Function):
     """SMPLModel.forward without the camera tail, with thmr_smpl_backward as its backward."""
 
