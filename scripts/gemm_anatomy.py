@@ -7,7 +7,7 @@ general one, and prints one JSON line per case:
       so almost only the fixed per-tile cost is left);
   (b) median, p90 and mean of each phase per tile from the kernel's %globaltimer timeline (GemmParams::timeline):
       wait = tile start -> first full barrier, mma = -> last wgmma retired, epilogue = -> epilogue done (for the
-      TMA-stored fp16 kinds: the tile's stores issued, not completed);
+      TMA-stored kinds: the tile's stores issued, or handed to the residual kind's reduction thread, not completed);
   (c) torch.matmul fp16 at the same M, N, K, with no epilogue, as the card's own yardstick for these shapes;
   (d) card name, power limit and SM clocks, read in the same run.
 

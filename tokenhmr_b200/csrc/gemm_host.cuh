@@ -8,7 +8,9 @@ namespace thmr {
 
 struct GemmPlan {
   CUtensorMap tmA, tmB;
-  CUtensorMap tmC;   // out16, box 64 x 64, SWIZZLE_128B: the TMA stores of the fp16 kinds (zero for the other plans)
+  // TMA-stored kinds, SWIZZLE_128B (zero for the other plans): out16, box 64 x 64 (fp16 kinds), or out32 = the
+  // residual, box 64 rows x 32 fp32 (residual kind: its loads and its stores)
+  CUtensorMap tmC;
   GemmParams p;
   int bn;
   int grid;
@@ -52,8 +54,8 @@ struct GemmDesc {
 // overhead, plus the epilogue.  The epilogue terms are fitted to the ViT GEMMs (M = 12288) on an H100 80GB HBM3 (700 W
 // power limit; scripts/gemm_anatomy.py, per-tile timeline), so that the model picks the measured-faster width at all
 // five of them.  Of the specialised epilogue kinds (block_n 128 / 256 only), the TMA-stored fp16 ones hold the
-// consumers 0.8-2.3 us per 128 columns (~2500 cycles), the fp32 residual one ~7 us (~12000 cycles: it reads and writes
-// 8 bytes per element); 256 wins at all five either way.  The general epilogue costs ~30 us per 128 x 256 tile (eight
+// consumers 0.8-2.3 us per 128 columns (~2500 cycles), the fp32 residual one ~5 us at block_n 256 (~9000 cycles: its
+// reductions of every SM drain through L2 at once) and ~3 us at 128; 256 wins at all five either way.  The general epilogue costs ~30 us per 128 x 256 tile (eight
 // 32-column chunks) against ~7 us per 128 x 128 tile; the narrower tiles are scaled from 128.  The row arg-min
 // epilogue (VQ) is not staged and is not charged.
 inline int pick_bn(int M, int N, int K, bool staged_epilogue, int epi_kind, int force) {
@@ -72,7 +74,7 @@ inline int pick_bn(int M, int N, int K, bool staged_epilogue, int epi_kind, int 
     const double feed = (128.0 + bn) * 128.0 / 32.0;
     const double epilogue = !staged_epilogue                                 ? 0.0
                             : bn >= 128 && gemm_epi_tma_store(epi_kind)       ? 2500.0 * bn / 128
-                            : bn >= 128 && epi_kind == kEpiBiasResidF32       ? 12000.0 * bn / 128
+                            : bn >= 128 && epi_kind == kEpiBiasResidF32       ? 9000.0 * bn / 128
                             : bn == 256                                       ? 55000.0
                                                                               : 7000.0 * bn / 128;
     const double cost = waves * (num_kb * ((mma > feed ? mma : feed) + 40.0) + epilogue);
@@ -103,9 +105,11 @@ inline int pick_bn_fp8(int M, int N, int K) {
   return best;
 }
 
-// Epilogue kind of a plain fp16 GEMM: a specialised kind (gemm_epilogue_kind) where the descriptor asks for exactly its
-// operations and every base and pitch it touches allows 16-byte row vectors, else kEpiGeneral.  Only the 128- and
-// 256-wide tiles, where the ViT's GEMMs run, have the specialised kernels.
+// Epilogue kind of a plain fp16 GEMM: a specialised kind where the descriptor asks for exactly its operations and every
+// base and pitch it touches allows 16-byte row vectors (the TMA kinds need that of their tensor maps), else kEpiGeneral.
+// The residual kind also needs the residual to alias out32 (resid == out32, ldr == ld32), as at every call site of the
+// engine: one tensor map then serves its loads and its stores.  Only the 128- and 256-wide tiles, where the ViT's GEMMs
+// run, have the specialised kernels.
 inline int gemm_pick_epi(const GemmDesc& d, int bn, int cluster) {
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   if ((bn != 128 && bn != 256) || cluster != 1 || d.argmin_out || d.resid_mod || d.seq_pitch || d.act32 || !al16(d.bias))
@@ -114,8 +118,8 @@ inline int gemm_pick_epi(const GemmDesc& d, int bn, int cluster) {
     if (d.act == kActNone) return d.bias ? kEpiBiasF16 : kEpiF16;
     if (d.act == kActGelu && d.bias) return kEpiBiasGeluF16;
   }
-  if (d.out32 && !d.out16 && d.resid && d.bias && d.act == kActNone && d.ld32 % 4 == 0 && al16(d.out32) &&
-      d.ldr % 4 == 0 && al16(d.resid))
+  if (d.out32 && !d.out16 && d.resid == d.out32 && d.ldr == d.ld32 && d.bias && d.act == kActNone &&
+      d.ld32 % 4 == 0 && al16(d.out32))
     return kEpiBiasResidF32;
   return kEpiGeneral;
 }
@@ -209,8 +213,12 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
              "gemm: epilogue kind %d does not fit this GEMM (its kind is %d)", d.force_epi - 1, plan->epi);
   if (d.force_epi) plan->epi = d.force_epi - 1;
   memset(&plan->tmC, 0, sizeof(plan->tmC));
-  if (gemm_epi_tma_store(plan->epi))   // gemm_pick_epi checked the 16-byte base and pitch TMA needs
+  // gemm_pick_epi checked the 16-byte base and pitch TMA needs
+  if (gemm_epi_tma_store(plan->epi))
     THMR_TRY(make_tmap_2d_f16(&plan->tmC, d.out16, d.M, d.N, d.ld16, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B));
+  if (plan->epi == kEpiBiasResidF32)
+    THMR_TRY(make_tmap_2d(&plan->tmC, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out32, d.M, d.N, d.ld32, 64, 32,
+                          CU_TENSOR_MAP_SWIZZLE_128B));
   const long tiles_m = (d.M + kGemmBM * cluster - 1) / (kGemmBM * cluster);
   const long tiles = d.argmin_out ? tiles_m : tiles_m * ((d.N + bn - 1) / bn);
   // the CTAs of a wave should share tiles of the larger operand (TileIter)
@@ -222,8 +230,8 @@ inline int gemm_make_plan(const GemmDesc& d, GemmPlan* plan) {
 
 template <int BN, int STAGES, int CLUSTER = 1, bool FP8 = false, int EPI = kEpiGeneral, bool TIMELINE = false>
 inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
-  using S = GemmSmem<BN, STAGES, FP8>;
-  static_assert(S::kTotal <= 232448, "GEMM shared memory exceeds 227 KB");
+  using S = GemmSmem<BN, STAGES, FP8, EPI>;
+  static_assert(S::kTotal <= kGemmSmemLimit, "GEMM shared memory exceeds 227 KB");
   static bool configured = false;
   if (!configured) {
     THMR_CUDA(cudaFuncSetAttribute(gemm_f16_tn_kernel<BN, STAGES, CLUSTER, FP8, EPI, TIMELINE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -247,14 +255,25 @@ inline int gemm_launch_t(const GemmPlan& plan, cudaStream_t stream) {
   return THMR_OK;
 }
 
-template <int BN, int STAGES, bool TIMELINE>
+// Operand ring depth of the 128- and 256-wide fp16 kernels; the residual kind's ring (GemmSmem::kResidBufs) takes
+// what is left.  At block_n 128 the residual kind gives up one stage so that its ring holds the whole tile (4 boxes per
+// warpgroup instead of 2); at 256 it keeps all 4 stages (2 boxes): one stage fewer (5 boxes) slowed the main loop more
+// than it shortened the epilogue.  DESIGN.md §6 has the timelines this was chosen from.
+template <int BN, int EPI>
+constexpr int gemm_stages() {
+  return BN == 256 ? 4 : EPI == kEpiBiasResidF32 ? 5 : 6;
+}
+
+template <int BN, bool TIMELINE>
 inline int gemm_launch_epi(const GemmPlan& plan, cudaStream_t stream) {
   switch (plan.epi) {
-    case kEpiGeneral: return gemm_launch_t<BN, STAGES, 1, false, kEpiGeneral, TIMELINE>(plan, stream);
-    case kEpiF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiF16, TIMELINE>(plan, stream);
-    case kEpiBiasF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasF16, TIMELINE>(plan, stream);
-    case kEpiBiasGeluF16: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasGeluF16, TIMELINE>(plan, stream);
-    case kEpiBiasResidF32: return gemm_launch_t<BN, STAGES, 1, false, kEpiBiasResidF32, TIMELINE>(plan, stream);
+    case kEpiGeneral: return gemm_launch_t<BN, gemm_stages<BN, kEpiGeneral>(), 1, false, kEpiGeneral, TIMELINE>(plan, stream);
+    case kEpiF16: return gemm_launch_t<BN, gemm_stages<BN, kEpiF16>(), 1, false, kEpiF16, TIMELINE>(plan, stream);
+    case kEpiBiasF16: return gemm_launch_t<BN, gemm_stages<BN, kEpiBiasF16>(), 1, false, kEpiBiasF16, TIMELINE>(plan, stream);
+    case kEpiBiasGeluF16:
+      return gemm_launch_t<BN, gemm_stages<BN, kEpiBiasGeluF16>(), 1, false, kEpiBiasGeluF16, TIMELINE>(plan, stream);
+    case kEpiBiasResidF32:
+      return gemm_launch_t<BN, gemm_stages<BN, kEpiBiasResidF32>(), 1, false, kEpiBiasResidF32, TIMELINE>(plan, stream);
   }
   return fail(THMR_ERR_INVALID, "gemm: unsupported epilogue kind %d", plan.epi);
 }
@@ -269,8 +288,8 @@ inline int gemm_launch_plain(const GemmPlan& plan, cudaStream_t stream) {
   }
   if (plan.cluster == 2) return gemm_launch_t<256, 4, 2>(plan, stream);
   switch (plan.bn) {
-    case 256: return gemm_launch_epi<256, 4, false>(plan, stream);
-    case 128: return gemm_launch_epi<128, 6, false>(plan, stream);
+    case 256: return gemm_launch_epi<256, false>(plan, stream);
+    case 128: return gemm_launch_epi<128, false>(plan, stream);
     case 64: return gemm_launch_t<64, 8>(plan, stream);
     case 32: return gemm_launch_t<32, 8>(plan, stream);
   }
@@ -284,7 +303,7 @@ inline int gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
   if constexpr (TIMELINE) {
     THMR_CHECK(!plan.fp8 && plan.cluster == 1 && (plan.bn == 128 || plan.bn == 256),
                "gemm timeline: fp16 block_n 128 / 256 only (block_n %d)", plan.bn);
-    return plan.bn == 256 ? gemm_launch_epi<256, 4, true>(plan, stream) : gemm_launch_epi<128, 6, true>(plan, stream);
+    return plan.bn == 256 ? gemm_launch_epi<256, true>(plan, stream) : gemm_launch_epi<128, true>(plan, stream);
   } else {
     THMR_CHECK(plan.epi == kEpiGeneral || (plan.bn >= 128 && plan.cluster == 1 && !plan.fp8),
                "gemm: epilogue kind %d at block_n %d", plan.epi, plan.bn);

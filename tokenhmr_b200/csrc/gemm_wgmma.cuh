@@ -5,6 +5,8 @@
 //   warps 0-3 : consumer warpgroup 0, rows 0..63 of the 128-row tile    wgmma m64nBNk16, then the epilogue
 //   warps 4-7 : consumer warpgroup 1, rows 64..127
 //   warps 8-11: producer warpgroup; one thread issues the TMA loads  global -> 128B-swizzled smem ring of STAGES k-blocks
+//               (residual kind: one thread each of warps 9 and 10 issues the TMA reductions of consumer
+//               warpgroup 0 / 1)
 //
 // setmaxnreg moves registers from the producer warpgroup (40 per thread) to the consumers (232), so that a 64 x 256
 // fp32 accumulator tile (128 registers per thread) and the epilogue fit without spilling.
@@ -19,8 +21,9 @@
 // whole row segments (gemm_epilogue_rows); it handles alpha scale, bias, a residual (may alias out32: same element,
 // same thread), residual tables, padded-sequence masking, activations, fp32 and / or fp16 outputs.  The fp16-output
 // epilogue kinds instead hand their finished tiles to TMA stores and go straight on to the next tile
-// (gemm_epilogue_f16_tma).  The row-argmin modes of the VQ nearest-code search work straight from the accumulator
-// registers.
+// (gemm_epilogue_f16_tma); so does the in-place fp32 residual kind, whose alpha * acc + bias two more producer threads
+// add into the residual with TMA reductions (gemm_resid_thread, gemm_epilogue_resid_tma).  The
+// row-argmin modes of the VQ nearest-code search work straight from the accumulator registers.
 //
 // The same kernel runs the implicit-GEMM Conv1d (k=3, dilated) of the pose-token decoder: k-blocks are
 // grouped in "taps", each tap reads the A rows shifted by a row offset (TMA zero-fills out-of-range rows).
@@ -37,10 +40,10 @@ enum : int { kActNone = 0, kActGelu = 1, kActRelu = 2 };
 //   kEpiF16           alpha * acc -> fp16                          decoder to_kv   (gemm_epilogue_f16_tma)
 //   kEpiBiasF16       alpha * acc + bias -> fp16                   QKV             (gemm_epilogue_f16_tma)
 //   kEpiBiasGeluF16   GELU(alpha * acc + bias) -> fp16             fc1             (gemm_epilogue_f16_tma)
-//   kEpiBiasResidF32  alpha * acc + bias + resid -> fp32           proj, fc2 (resid aliases out32; gemm_epilogue_resid)
+//   kEpiBiasResidF32  alpha * acc + bias + resid -> fp32           proj, fc2 (resid aliases out32; gemm_epilogue_resid_tma)
 enum : int { kEpiGeneral = 0, kEpiF16 = 1, kEpiBiasF16 = 2, kEpiBiasGeluF16 = 3, kEpiBiasResidF32 = 4 };
 
-// The fp16-output kinds store their tiles with TMA through GemmPlan::tmC.
+// The fp16-output kinds store their tiles with TMA through GemmPlan::tmC; the residual kind adds into x through it.
 constexpr bool gemm_epi_tma_store(int epi) { return epi == kEpiF16 || epi == kEpiBiasF16 || epi == kEpiBiasGeluF16; }
 
 struct GemmParams {
@@ -96,7 +99,7 @@ struct GemmParams {
   int ld8s;
   // per-tile phase timeline (gemm_f16_tn_kernel<..., TIMELINE = true>, test probe only): lane 0 of each consumer
   // warpgroup writes four %globaltimer stamps per tile into timeline[cta][slot][wg][4] (tile start, first full barrier
-  // passed, last wgmma retired, epilogue done -- for the TMA-stored fp16 kinds: the tile's stores issued, not completed)
+  // passed, last wgmma retired, epilogue done -- for the TMA-stored kinds: the tile's stores issued, not completed)
   // for the CTA's first timeline_slots tiles, and %smid into timeline_sm[cta]
   unsigned long long* timeline;
   int timeline_slots;
@@ -147,21 +150,34 @@ constexpr int gemm_chunk() { return BN == 64 || BN == 128 ? 64 : 32; }
 template <bool FP8>
 constexpr int gemm_bk() { return FP8 ? 128 : kGemmBK; }
 
-template <int BN, int STAGES, bool FP8 = false>
+// Largest dynamic shared memory of one CTA on sm_90 (227 KB).
+constexpr uint32_t kGemmSmemLimit = 232448;
+// One box of the residual kind's ring (gemm_epilogue_resid_tma): 64 rows x 32 fp32 columns, one 128-byte swizzle row each.
+constexpr uint32_t kResidBoxBytes = 64 * 32 * 4;
+
+template <int BN, int STAGES, bool FP8 = false, int EPI = kEpiGeneral>
 struct GemmSmem {
   static constexpr uint32_t kABytes = kGemmBM * kGemmBK * 2;
   static constexpr uint32_t kBBytes = BN * kGemmBK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;   // multiple of 1024: every operand tile stays swizzle-aligned
-  // epilogue staging, 16 KB per warpgroup: a 64 x gemm_chunk block of fp32 accumulators (general and residual
-  // epilogues) or a 64 x 128 fp16 output tile, two 128B-swizzled TMA store boxes (fp16 kinds), so 1024-byte aligned
   static constexpr uint32_t kEpiOffset = STAGES * kStageBytes;
-  static constexpr uint32_t kEpiWgBytes = 64 * 128 * 2;
-  static_assert(64 * gemm_chunk<BN>() * 4 <= kEpiWgBytes, "fp32 staging chunk exceeds the warpgroup's block");
+  // residual kind: per warpgroup a ring of kResidBufs 64 x 32 fp32 boxes, as many as fit next to the operand ring (at
+  // most one tile's worth); they hold alpha * acc + bias until the TMA reductions have read it
+  static constexpr int kResidFit = static_cast<int>((kGemmSmemLimit - kEpiOffset - 256 - 1024) / (2 * kResidBoxBytes));
+  static constexpr int kResidBufs = EPI != kEpiBiasResidF32 ? 0 : kResidFit < BN / 32 ? kResidFit : BN / 32;
+  static_assert(EPI != kEpiBiasResidF32 || kResidBufs >= 2, "residual ring needs two boxes per warpgroup");
+  // otherwise epilogue staging, 16 KB per warpgroup: a 64 x gemm_chunk block of fp32 accumulators (general epilogue) or
+  // a 64 x 128 fp16 output tile, two 128B-swizzled TMA store boxes (fp16 kinds).  Either way 1024-byte aligned.
+  static constexpr uint32_t kEpiWgBytes = EPI == kEpiBiasResidF32 ? kResidBufs * kResidBoxBytes : 64 * 128 * 2;
+  static_assert(EPI == kEpiBiasResidF32 || 64 * gemm_chunk<BN>() * 4 <= kEpiWgBytes,
+                "fp32 staging chunk exceeds the warpgroup's block");
   static constexpr uint32_t kEpiBytes = 2 * kEpiWgBytes;
   // FP8: the 128 activation scales of each stage's k-block ride the same ring, outside the swizzled operand tiles
   static constexpr uint32_t kScaleOffset = kEpiOffset + kEpiBytes;
   static constexpr uint32_t kScaleBytes = FP8 ? STAGES * kGemmBM * 4 : 0;
+  // mbarriers: full / empty per stage, then (residual kind) free / done per ring box of each warpgroup
   static constexpr uint32_t kBarOffset = kScaleOffset + kScaleBytes;
+  static_assert((2 * STAGES + 4 * kResidBufs) * 8 <= 256, "mbarriers exceed their 256 bytes");
   static constexpr uint32_t kRowScaleOffset = kBarOffset + 256;   // FP8 e4m3 output: 1 / scale of each tile row
   static constexpr uint32_t kRowScaleBytes = FP8 ? kGemmBM * 4 : 0;
   static constexpr uint32_t kTotal = kRowScaleOffset + kRowScaleBytes + 1024;  // alignment slack
@@ -386,104 +402,115 @@ __device__ __forceinline__ void gemm_epilogue_rows(const GemmParams& p, const fl
   }
 }
 
-// The octet of a partial column tile (col < N < col + 8) of gemm_epilogue_resid, element by element.
-__device__ __forceinline__ void gemm_epilogue_resid_tail(const GemmParams& p, const float (&v)[8], int row, int col) {
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    if (col + e >= p.N) break;
-    const float x = __fadd_rn(__fmul_rn(v[e], p.alpha), __ldg(p.bias + col + e));
-    const float r = p.resid[static_cast<size_t>(row) * p.ldr + col + e];
-    p.out32[static_cast<size_t>(row) * p.ld32 + col + e] = __fadd_rn(x, r);
+// Ring position of a warpgroup's residual boxes (kEpiBiasResidF32): the reduction thread and the consumers walk the
+// same sequence of boxes, so each side keeps its own copy.
+struct RingPos {
+  int slot = 0;
+  uint32_t phase = 0;
+  template <int NB>
+  __device__ __forceinline__ void next() {
+    if (++slot == NB) { slot = 0; phase ^= 1; }
   }
+};
+
+// The boxes of one consumer warpgroup in the order its residual epilogue takes them: per tile, one 64 x 32 box of rows
+// m0w .. m0w + 63 per 32 columns.  Boxes past N are skipped, and so are the tiles in which the warpgroup has no rows
+// (m0w >= M); TMA clips the reductions past [M, N].
+template <int BN>
+struct ResidBoxIter {
+  TileIter it;
+  int row_off, M, N, c = 0;
+  __device__ ResidBoxIter(const TileIter& t, int ro, int m, int n) : it(t), row_off(ro), M(m), N(n) { skip(); }
+  __device__ bool valid() const { return it.valid(); }
+  __device__ int m0w() const { return it.m0(kGemmBM) + row_off; }
+  __device__ int col() const { return it.n0(BN) + 32 * c; }
+  __device__ void skip() {
+    while (it.valid() && m0w() >= M) it.next();
+  }
+  __device__ void next() {
+    if (++c == BN / 32 || col() >= N) {
+      c = 0;
+      it.next();
+      skip();
+    }
+  }
+};
+
+// Reduction thread of one consumer warpgroup (kEpiBiasResidF32; one thread of the producer warpgroup each).  It owns the
+// TMA side of the warpgroup's ring of NB boxes: for each box in turn it waits until the consumers have written
+// alpha * acc + bias into it, adds the box into x with a TMA reduction (x += box, in L2), and hands the previous box
+// back to the consumers as soon as its reduction has read it.  The residual is never loaded into the SM, and the waits
+// on the reductions are this thread's alone, so the consumers only wait for a free box.
+template <int BN, int NB>
+__device__ __forceinline__ void gemm_resid_thread(const CUtensorMap* tm, uint32_t ring, uint64_t* free_bar,
+                                                  uint64_t* done, ResidBoxIter<BN> it) {
+  for (int s = 0; s < NB; ++s) mbar_arrive(&free_bar[s]);
+  RingPos rp;
+  int prev = -1;
+  for (; it.valid(); it.next()) {
+    mbar_wait(&done[rp.slot], rp.phase);
+    tma_reduce_add_2d(tm, ring + rp.slot * kResidBoxBytes, it.col(), it.m0w());
+    tma_store_commit();
+    if (prev >= 0) {
+      tma_store_wait_read<1>();
+      mbar_arrive(&free_bar[prev]);
+    }
+    prev = rp.slot;
+    rp.next<NB>();
+  }
+  // the reductions complete (and stop reading the ring) before the CTA exits
+  tma_store_wait<0>();
 }
 
-// Element-wise epilogue of one consumer warpgroup for kEpiBiasResidF32: the staging and the row walk of
-// gemm_epilogue_rows and the same values element for element, but only the kind's operations are compiled, and the
-// chunks go through one rolled loop, so that the walk is emitted once instead of once per chunk.  Only the fragment
-// staging is unrolled per chunk (a uniform branch picks it), since it indexes registers.  The plan (gemm_make_plan)
-// guarantees 16-byte aligned bases and pitches for the bias, the residual and out32.
-template <int BN>
-__device__ __forceinline__ void gemm_epilogue_resid(const GemmParams& p, const float (&acc)[BN / 2], uint32_t stage,
-                                                    int m0w, int n0, int M_eff, uint32_t bar_id) {
-  constexpr int CH = gemm_chunk<BN>();
-  constexpr int OCT = CH / 8;
-  constexpr int ITEMS = OCT / 2;
+// Epilogue of one consumer warpgroup for kEpiBiasResidF32, x = alpha * acc + bias + x in place (out32 aliases the
+// residual; GemmPlan::tmC maps it): its 64 rows x BN columns, rows m0w.. of the output, one 64 x 32 box of the ring
+// per 32 columns.  Each thread writes alpha * acc + bias, rounded step by step as gemm_epilogue_rows does, from the
+// accumulator fragment into a free box (SWIZZLE_128B: row r is 128 bytes, 16-byte unit u at u ^ (r % 8)); each warp
+// then hands the box to gemm_resid_thread, whose TMA reduction adds it into x, and goes on without waiting.  fp32
+// addition is commutative, so x + v equals the general epilogue's v + x bit for bit, except that the reduction
+// flushes a subnormal x, v or sum (|.| < 2^-126) to zero.
+// The fragment's rows r and r ^ 1 hit the same two units of a column group, so odd rows take the column groups in the
+// order 2, 3, 0, 1: the sixteen 64-bit stores of a half-warp (four rows x 32 bytes) then fall on distinct banks.
+template <int BN, int NB>
+__device__ __forceinline__ void gemm_epilogue_resid_tma(const GemmParams& p, const float (&acc)[BN / 2], uint32_t ring,
+                                                        uint64_t* free_bar, uint64_t* done, RingPos& rp, int n0) {
   const int lane = threadIdx.x & 31;
-  const int w4 = (threadIdx.x >> 5) & 3;
-  const int fr = w4 * 16 + (lane >> 2);
-  const int fswz = (((lane >> 2) & 3) << 1) | ((lane >> 4) & 1);
-  const int rswz = ((lane & 3) << 1) | ((lane >> 2) & 1);
+  // fragment: rows fr, fr + 8 of the warpgroup (both = lane / 4 mod 8), columns 8 j + c0 + {0, 1}
+  const int fr = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const int swz = (lane >> 2) & 7;
+  const int jx = (lane & 4) ? 2 : 0;   // odd rows: column group jj ^ 2
 #pragma unroll 1
-  for (int c = 0; c < BN / CH; ++c) {
+  for (int c = 0; c < BN / 32; ++c) {
+    const int nc = n0 + 32 * c;
+    if (nc >= p.N) break;
+    mbar_wait(&free_bar[rp.slot], rp.phase);
+    const uint32_t box = ring + rp.slot * kResidBoxBytes;
 #pragma unroll
-    for (int cc = 0; cc < BN / CH; ++cc)
-      if (cc == c) gemm_stage_chunk<BN>(acc, cc, stage, fr, fswz, lane);
-    named_barrier_sync(bar_id, 128);
-
-    // item k: row 8 (w4 + 4 (k % 2)) + lane % 8 of the warpgroup, octet 4 (k / 2) + lane / 8 of the chunk
-    const int ccol = n0 + c * CH + 8 * (lane >> 3);
-    float bias[ITEMS / 2][8];
-    float res[ITEMS][8];
-    if constexpr (ITEMS != 2) {
+    for (int cc = 0; cc < BN / 32; ++cc) {
+      if (cc != c) continue;   // a uniform branch: the fragment is indexed by constants
 #pragma unroll
-      for (int ob = 0; ob < ITEMS / 2; ++ob) {
-        const int col = ccol + 32 * ob;
-        if (col + 8 <= p.N) {
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-          const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
-          bias[ob][0] = b0.x; bias[ob][1] = b0.y; bias[ob][2] = b0.z; bias[ob][3] = b0.w;
-          bias[ob][4] = b1.x; bias[ob][5] = b1.y; bias[ob][6] = b1.z; bias[ob][7] = b1.w;
+      for (int t = 0; t < 4; ++t) {
+        const int jj = t ^ jx;
+        const int col = nc + 8 * jj + c0;
+        // columns past N are clipped by the reduction, so their bias may be any value
+        const float b0 = __ldg(p.bias + min(col, p.N - 1));
+        const float b1 = __ldg(p.bias + min(col + 1, p.N - 1));
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int a = 4 * (4 * cc + t) + 2 * i, a2 = 4 * (4 * cc + (t ^ 2)) + 2 * i;
+          const float v0 = jx ? acc[a2] : acc[a];
+          const float v1 = jx ? acc[a2 + 1] : acc[a + 1];
+          sts_f32x2(box + (fr + 8 * i) * 128 + (((2 * jj + (c0 >> 2)) ^ swz) << 4) + 4 * (c0 & 3),
+                    __fadd_rn(__fmul_rn(v0, p.alpha), b0), __fadd_rn(__fmul_rn(v1, p.alpha), b1));
         }
       }
     }
-    // all residual loads of the chunk before any of its stores
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-      const int row = m0w + 8 * (w4 + 4 * (k & 1)) + (lane & 7);
-      const int col = ccol + 32 * (k >> 1);
-      if (row < M_eff && col + 8 <= p.N) {
-        const float* r = p.resid + static_cast<size_t>(row) * p.ldr + col;
-        const float4 x0 = *reinterpret_cast<const float4*>(r);
-        const float4 x1 = *reinterpret_cast<const float4*>(r + 4);
-        res[k][0] = x0.x; res[k][1] = x0.y; res[k][2] = x0.z; res[k][3] = x0.w;
-        res[k][4] = x1.x; res[k][5] = x1.y; res[k][6] = x1.z; res[k][7] = x1.w;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-      const int lr = 8 * (w4 + 4 * (k & 1)) + (lane & 7);
-      const int oct = 4 * (k >> 1) + (lane >> 3);
-      const int row = m0w + lr;
-      const int col = ccol + 32 * (k >> 1);
-      if (row >= M_eff || col >= p.N) continue;
-      float v[8];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int u = 2 * oct + h;
-        const float4 s = lds_f32x4(stage + 4 * (lr * CH + (((u & ~7) | ((u ^ rswz) & 7)) << 2)));
-        v[4 * h] = s.x; v[4 * h + 1] = s.y; v[4 * h + 2] = s.z; v[4 * h + 3] = s.w;
-      }
-      if (col + 8 > p.N) {
-        gemm_epilogue_resid_tail(p, v, row, col);
-        continue;
-      }
-      if constexpr (ITEMS == 2) {
-        // 128 accumulators stay live across the rolled chunk loop: the 32-column chunks of BN = 256 have no registers
-        // left to hold the bias from before the residual loads, so it is read here
-        const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-        const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
-        bias[0][0] = b0.x; bias[0][1] = b0.y; bias[0][2] = b0.z; bias[0][3] = b0.w;
-        bias[0][4] = b1.x; bias[0][5] = b1.y; bias[0][6] = b1.z; bias[0][7] = b1.w;
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        v[e] = __fadd_rn(__fadd_rn(__fmul_rn(v[e], p.alpha), bias[k >> 1][e]), res[k][e]);
-      float4* o = reinterpret_cast<float4*>(p.out32 + static_cast<size_t>(row) * p.ld32 + col);
-      o[0] = make_float4(v[0], v[1], v[2], v[3]);
-      o[1] = make_float4(v[4], v[5], v[6], v[7]);
-    }
-    // the next chunk (or tile) overwrites the staging block
-    named_barrier_sync(bar_id, 128);
+    // the values become visible to the TMA unit (async proxy) before the reduction thread hands them to it
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&done[rp.slot]);
+    rp.next<NB>();
   }
 }
 
@@ -584,8 +611,9 @@ template <int BN, int STAGES, int CLUSTER, bool FP8 = false, int EPI = kEpiGener
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-  using S = GemmSmem<BN, STAGES, FP8>;
+  using S = GemmSmem<BN, STAGES, FP8, EPI>;
   constexpr int BK = gemm_bk<FP8>();
+  constexpr int NB = S::kResidBufs;
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
   static_assert(CLUSTER == 1 || (CLUSTER == 2 && BN >= 128), "cluster pairs split B in two halves of >= 64 rows");
   static_assert(!FP8 || (CLUSTER == 1 && (BN == 64 || BN == 128)), "FP8: two accumulator sets fit at BN <= 128");
@@ -596,6 +624,9 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
+  // residual kind: the ring boxes' free (reduction has read it) and done (values written) barriers, NB per warpgroup
+  uint64_t* rfree_bar = empty_bar + STAGES;
+  uint64_t* rdone_bar = rfree_bar + 2 * NB;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -621,12 +652,16 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kGemmConsumerWarps * CLUSTER);   // one arrive per consumer warp of the cluster
     }
+    for (int b = 0; b < 2 * NB; ++b) {
+      mbar_init(&rfree_bar[b], 1);   // the reduction thread's arrive
+      mbar_init(&rdone_bar[b], 4);   // one arrive per warp of the consumer warpgroup
+    }
     fence_mbar_init();
   }
   if (warp == kWarpTma && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if constexpr (gemm_epi_tma_store(EPI)) tma_prefetch_desc(&tmC);
+    if constexpr (gemm_epi_tma_store(EPI) || EPI == kEpiBiasResidF32) tma_prefetch_desc(&tmC);
   }
   if constexpr (CLUSTER == 2) cluster_sync_all();   // the peer's barriers are initialised before any multicast or arrive
   else __syncthreads();
@@ -661,6 +696,14 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
+    if constexpr (EPI == kEpiBiasResidF32) {
+      // warps kWarpTma + 1 and + 2: the reduction threads of consumer warpgroups 0 and 1
+      const int rw = warp - kWarpTma - 1;
+      if ((rw == 0 || rw == 1) && lane == 0)
+        gemm_resid_thread<BN, NB>(
+            &tmC, smem_u32(smem + S::kEpiOffset + rw * S::kEpiWgBytes), rfree_bar + rw * NB, rdone_bar + rw * NB,
+            ResidBoxIter<BN>(TileIter(tiles_m, tiles_n, false, p.m_fast != 0, tile0, tile_step), 64 * rw, M_eff, p.N));
+    }
     if constexpr (CLUSTER == 2) cluster_sync_all();
     return;
   }
@@ -685,6 +728,7 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint32_t phase = 0;
   float acc[BN / 2];
   float tile[FP8 ? BN / 2 : 1];   // FP8: the current k-block's products
+  RingPos rp;   // residual kind: this warpgroup's position in its ring
 
   // a consumed stage is released to the producers of every CTA of the cluster
   auto release = [&](int s) {
@@ -834,7 +878,8 @@ gemm_f16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       if (p.out8) gemm_row_scales_e4m3<BN>(p, acc, m0, n0, r0, c0, wg, M_eff, row_inv);
       gemm_epilogue_rows<BN, true>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg, vec_r, vec32, vec16, row_inv);
     } else if constexpr (EPI == kEpiBiasResidF32) {
-      gemm_epilogue_resid<BN>(p, acc, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
+      if (m0 + wg * 64 < M_eff)
+        gemm_epilogue_resid_tma<BN, NB>(p, acc, epi_stage, rfree_bar + wg * NB, rdone_bar + wg * NB, rp, n0);
     } else if constexpr (EPI != kEpiGeneral) {
       gemm_epilogue_f16_tma<BN, EPI>(p, acc, &tmC, epi_stage, m0 + wg * 64, n0, M_eff, 1 + wg);
     } else {

@@ -174,6 +174,14 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem
                : "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
+// 2D tiled reduction shared -> global: adds the box element-wise into the tensor (global += smem), clipped at the
+// tensor's bounds.  fp32 adds round to nearest even, and flush subnormal inputs and results to zero.
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, uint32_t smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               :
+               : "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
