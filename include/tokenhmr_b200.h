@@ -448,6 +448,10 @@ typedef struct thmr_config {
                  * Not with strict (THMR_ERR_INVALID). */
 } thmr_config;
 
+/* SMPL heads (thmr_engine_create_head) */
+#define THMR_HEAD_TOKEN 0
+#define THMR_HEAD_REGRESSION 1
+
 /* Weight pointers, packed by the host loader (tokenhmr_b200/weights.py) from the reference state_dicts.
  * "w" matrices are f16 [out,in] (nn.Linear layout); vectors are fp32. */
 typedef struct thmr_vit_block {
@@ -498,15 +502,16 @@ typedef struct thmr_weights {
   const float* token0;                         /* [E] = to_token_embedding.bias + pos_embedding */
   const void* kv_w;                            /* [dec_depth * 2*inner, D]: to_kv of all layers stacked */
   const thmr_dec_layer* dec_host;              /* host array [dec_depth] */
-  const void* readout_w; const float* readout_b; /* [32, E]: grot(6) hands(12) shape(10) cam(3) + 1 zero row */
+  const void* readout_w; const float* readout_b; /* token head [32, E]: grot(6) hands(12) shape(10) cam(3) + 1 zero
+                                                  * row; regression head [160, E]: pose(144) shape(10) cam(3) + 3 */
   const float *init_pose, *init_betas, *init_cam; /* [144], [10], [3] */
-  /* token classifier */
+  /* token classifier (token head only) */
   const void* mt_w; const float* mt_b; const float *mt_ln_g, *mt_ln_b; /* Linear E -> T*H, LN(T*H) */
   const thmr_mixer_block* mixer_host;          /* host array [cls_blocks] */
   const void* mn_w; const float* mn_b; const float *mn_ln_g, *mn_ln_b; /* Linear H->H, LN(H) */
   const void* cls_w; const float* cls_b;       /* [classes, H] */
-  /* tokenizer */
-  const void* codebook_t;                      /* f16 [code_dim, nb_code] */
+  /* tokenizer (token head only) */
+  const void* codebook_t;                     /* f16 [code_dim, nb_code] */
   thmr_conv conv_in;                           /* code_dim -> W */
   thmr_conv conv_up[8];                        /* after each Upsample */
   thmr_conv res_conv1[8], res_conv2[8];        /* Resnet1D blocks in stored order (dilation rate^(depth-1) ... 1) */
@@ -516,7 +521,7 @@ typedef struct thmr_weights {
 } thmr_weights;
 
 typedef struct thmr_outputs {                  /* all fp32, caller-allocated; any pointer may be NULL */
-  float* cls_logits_softmax;  /* [B,160,2048] */
+  float* cls_logits_softmax;  /* [B,160,2048]; token head only: must be NULL for THMR_HEAD_REGRESSION */
   float* pred_cam;            /* [B,3] */
   float* rotmats;             /* [B,24,3,3]: global_orient = [:, :1], body_pose = [:, 1:] */
   float* betas;               /* [B,10] */
@@ -532,6 +537,15 @@ typedef struct thmr_outputs {                  /* all fp32, caller-allocated; an
 } thmr_outputs;
 
 int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr_smpl* smpl, thmr_engine** out);
+/* thmr_engine_create with a choice of SMPL head [heads/__init__.py:4-13].  THMR_HEAD_TOKEN: SMPLTokenDecoderHead
+ * [token_head.py] with the token classifier and the tokenizer decoder (what thmr_engine_create builds).
+ * THMR_HEAD_REGRESSION: SMPLTransformerDecoderHead [smpl_head.py], HMR 2.0's head: the decoder's output token is read out
+ * by one linear layer into all 24 6D rotations, betas and camera; readout_w is then [160, E] = decpose(144) |
+ * decshape(10) | deccam(3) | 3 zero rows, the classifier and tokenizer pointers of thmr_weights are ignored (may be NULL)
+ * and the forward produces no cls_logits_softmax (a non-NULL thmr_outputs::cls_logits_softmax is THMR_ERR_INVALID).
+ * Works in every numeric mode. */
+int thmr_engine_create_head(const thmr_config* cfg, int head_type, const thmr_weights* w, const thmr_smpl* smpl,
+                            thmr_engine** out);
 void thmr_engine_destroy(thmr_engine* e);
 size_t thmr_engine_workspace_bytes(const thmr_engine* e, int max_batch);
 /* img fp32 [B,3,image_size,image_size] (batch['img']).  `workspace` must hold

@@ -60,6 +60,9 @@ class Config(Structure):
                 ("focal_length", c_float), ("strict", c_int), ("concurrent", c_int), ("fp8", c_int)]
 
 
+HEAD_TOKEN, HEAD_REGRESSION = 0, 1          # thmr_engine_create_head (THMR_HEAD_TOKEN / THMR_HEAD_REGRESSION)
+
+
 class VitBlock(Structure):
     _fields_ = [(n, c_void_p) for n in ("ln1_g", "ln1_b", "qkv_w", "qkv_b", "proj_w", "proj_b", "ln2_g", "ln2_b",
                                         "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
@@ -227,6 +230,7 @@ SIGNATURES = {
     "thmr_tokenhmr_loss_workspace_bytes": (c_size_t, [c_int]),
     "thmr_tokenhmr_loss": (c_int, [POINTER(LossDesc), c_void_p, c_void_p]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
+    "thmr_engine_create_head": (c_int, [POINTER(Config), c_int, POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),
     "thmr_engine_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "thmr_engine_forward": (c_int, [c_void_p, c_void_p, c_int, POINTER(Outputs), c_void_p, c_void_p]),

@@ -207,23 +207,38 @@ def _unsupported(what: str, got, want, ref: str):
     raise ThmrError(f"unsupported configuration: {what} = {got!r}; this engine implements {want} only ({ref})")
 
 
+REGRESSION_HEAD = "transformer_decoder"
+
+
 def validate_model_config(y: Dict[str, Any]) -> None:
     """Reject every reference variant the engine does not implement instead of silently running the release path.
     Defaults are the reference's own `.get()` defaults."""
     m = y.get("MODEL", {}) or {}
     head = m.get("SMPL_HEAD", {}) or {}
-    # build_smpl_head (heads/__init__.py:4-13): default 'hmr' raises in the reference too; only 'token' is built here
-    if "SMPL_HEAD" in m and head.get("TYPE", "hmr") != "token":
+    # build_smpl_head (heads/__init__.py:4-13): default 'hmr' raises in the reference too; 'token' and
+    # 'transformer_decoder' (HMR 2.0's regression head) are built here
+    if "SMPL_HEAD" in m and head.get("TYPE", "hmr") not in ("token", REGRESSION_HEAD):
         _unsupported("MODEL.SMPL_HEAD.TYPE", head.get("TYPE", "hmr"), "'token' (SMPLTokenDecoderHead)", "heads/__init__.py:4-13")
+    regression = "SMPL_HEAD" in m and head.get("TYPE") == REGRESSION_HEAD
+    # the regression head reads the same three keys at the same places as the token head (smpl_head.py lines)
     if int(head.get("IEF_ITERS", 1)) != 1:
-        _unsupported("MODEL.SMPL_HEAD.IEF_ITERS", head.get("IEF_ITERS"), "1 iteration", "token_head.py:86")
+        _unsupported("MODEL.SMPL_HEAD.IEF_ITERS", head.get("IEF_ITERS"), "1 iteration",
+                     "smpl_head.py:70" if regression else "token_head.py:86")
     if head.get("TRANSFORMER_INPUT", "zero") != "zero":
         _unsupported("MODEL.SMPL_HEAD.TRANSFORMER_INPUT", head.get("TRANSFORMER_INPUT"), "'zero' (constant query token)",
-                     "token_head.py:29,88-91")
+                     "smpl_head.py:21-24,72-75" if regression else "token_head.py:29,88-91")
     if head.get("JOINT_REP", "6d") != "6d":
-        _unsupported("MODEL.SMPL_HEAD.JOINT_REP", head.get("JOINT_REP"), "'6d'", "token_head.py:23-24")
+        _unsupported("MODEL.SMPL_HEAD.JOINT_REP", head.get("JOINT_REP"), "'6d'",
+                     "smpl_head.py:17-18,61-62" if regression else "token_head.py:23-24")
     tk = head.get("TOKENIZER", {}) or {}
-    if tk.get("TOKENIZER_TYPE", "Vanilla") not in ("Vanilla",):
+    # MODEL.SMPL_HEAD.TOKENIZER configures the token classifier and the tokenizer (token_head.py:25-26,45-47), which the
+    # regression head does not have (smpl_head.py:14-48) and HMR 2.0's configs do not carry: a yaml with both is a
+    # TokenHMR yaml whose TYPE was changed, and its token settings would go unused, so it is refused, not guessed at
+    if regression and "TOKENIZER" in head:
+        _unsupported("MODEL.SMPL_HEAD.TOKENIZER with TYPE 'transformer_decoder'", sorted(tk),
+                     "no TOKENIZER block for the regression head (it has no token classifier)",
+                     "smpl_head.py:14-48, token_head.py:25-26,45-47")
+    if not regression and tk.get("TOKENIZER_TYPE", "Vanilla") not in ("Vanilla",):
         _unsupported("MODEL.SMPL_HEAD.TOKENIZER.TOKENIZER_TYPE", tk.get("TOKENIZER_TYPE"), "'Vanilla'",
                      "token_classifier.py:12-20")
     dec = head.get("TRANSFORMER_DECODER", {}) or {}
@@ -247,9 +262,38 @@ def validate_model_config(y: Dict[str, Any]) -> None:
         _unsupported("SMPL.GENDER", smpl.get("GENDER"), "an SMPL .pkl gender", "smpl_wrapper.py:10")
 
 
+def infer_head(sd: Dict[str, torch.Tensor]) -> str:
+    """The SMPL head a checkpoint holds, from its keys: `smpl_head.decpose.weight` (npose, dec_dim) is the regression
+    head's pose read-out (smpl_head.py:32), `smpl_head.decpose.mixer_trans.*` the token head's classifier
+    (token_head.py:45, token_classifier.py:67-69)."""
+    from ._lib import ThmrError
+    regression = "smpl_head.decpose.weight" in sd and sd["smpl_head.decpose.weight"].dim() == 2
+    token = any(k.startswith("smpl_head.decpose.mixer_trans.") for k in sd)
+    if regression == token:
+        raise ThmrError("cannot tell the SMPL head from the checkpoint keys: expected either smpl_head.decpose.weight "
+                        "(MODEL.SMPL_HEAD.TYPE 'transformer_decoder') or smpl_head.decpose.mixer_trans.* ('token')"
+                        + (", found both" if token else ", found neither"))
+    return REGRESSION_HEAD if regression else "token"
+
+
 def validate_against_weights(cfg: TokenHMRConfig, sd: Dict[str, torch.Tensor], smpl: Dict[str, torch.Tensor]) -> None:
     """Shapes the files imply must agree with the configuration the engine is built for."""
     from ._lib import ThmrError
+    if cfg.head == REGRESSION_HEAD:
+        if any(k.startswith("smpl_head.decpose.mixer_trans.") for k in sd):
+            raise ThmrError("the configuration says MODEL.SMPL_HEAD.TYPE 'transformer_decoder' but the checkpoint holds "
+                            "a token head (smpl_head.decpose.mixer_trans.*)")
+        # decpose / decshape / deccam read the decoder's output token (smpl_head.py:32-34)
+        for name, rows in (("decpose", cfg.npose), ("decshape", cfg.num_betas), ("deccam", 3)):
+            w, b = sd.get(f"smpl_head.{name}.weight"), sd.get(f"smpl_head.{name}.bias")
+            if w is None or b is None:
+                raise ThmrError(f"regression head: smpl_head.{name}.weight / .bias missing from the checkpoint")
+            if tuple(w.shape) != (rows, cfg.dec_dim) or tuple(b.shape) != (rows,):
+                raise ThmrError(f"regression head: smpl_head.{name} is {tuple(w.shape)} but the engine reads "
+                                f"({rows}, {cfg.dec_dim}) (npose / betas / camera x dec_dim)")
+    elif "smpl_head.decpose.weight" in sd:
+        raise ThmrError("the configuration says MODEL.SMPL_HEAD.TYPE 'token' but the checkpoint holds a regression head "
+                        "(smpl_head.decpose.weight): build it with TokenHMRConfig(head='transformer_decoder')")
     cb = sd.get("tokenizer.quantizer.codebook")
     if cb is not None and tuple(cb.shape) != (cfg.token_class_num, cfg.code_dim):
         raise ThmrError(f"tokenizer codebook is {tuple(cb.shape)} but the classifier predicts {cfg.token_class_num} classes "
@@ -266,9 +310,11 @@ def validate_against_weights(cfg: TokenHMRConfig, sd: Dict[str, torch.Tensor], s
                       "(smpl_wrapper.py:22-23,37-39)")
 
 
-def config_from_files(model_cfg_yaml: Optional[str], arch: Optional[Dict[str, Any]] = None) -> TokenHMRConfig:
-    """model_config.yaml (MODEL.* of the yacs dump, models/__init__.py:6-17) + tokenizer hparams -> TokenHMRConfig."""
-    kw: Dict[str, Any] = {}
+def config_from_files(model_cfg_yaml: Optional[str], arch: Optional[Dict[str, Any]] = None,
+                      head: Optional[str] = None) -> TokenHMRConfig:
+    """model_config.yaml (MODEL.* of the yacs dump, models/__init__.py:6-17) + tokenizer hparams -> TokenHMRConfig.
+    `head`: the SMPL head when the yaml does not name one (MODEL.SMPL_HEAD.TYPE wins)."""
+    kw: Dict[str, Any] = {"head": head} if head else {}
     if model_cfg_yaml:
         import yaml
         with open(model_cfg_yaml) as f:
@@ -280,6 +326,8 @@ def config_from_files(model_cfg_yaml: Optional[str], arch: Optional[Dict[str, An
         if m.get("BBOX_SHAPE"):
             kw["crop_w"] = int(m["BBOX_SHAPE"][0])
         head = m.get("SMPL_HEAD", {})
+        if head.get("TYPE"):
+            kw["head"] = str(head["TYPE"])
         t = head.get("TOKENIZER", {})
         for src, dst in (("TOKEN_CODE_DIM", "code_dim"), ("TOKEN_NUM", "token_num"), ("TOKEN_CLASS_NUM", "token_class_num")):
             if src in t:
@@ -303,17 +351,27 @@ def load_tokenhmr(checkpoint_path: str, model_cfg: Optional[str] = None, tokeniz
                   device: str = "cuda:0", **engine_kw):
     """File-based counterpart of lib.models.load_tokenhmr (tokenhmr/lib/models/__init__.py:3-26): returns (model, cfg).
     Paths default to the reference's layout relative to the checkpoint (data/checkpoints/tokenizer.pth,
-    data/body_models/smpl, data/body_models/SMPL_to_J19.pkl)."""
+    data/body_models/smpl, data/body_models/SMPL_to_J19.pkl).
+    The SMPL head is the yaml's MODEL.SMPL_HEAD.TYPE, or without a yaml the one the checkpoint's keys hold
+    (infer_head); an HMR 2.0 checkpoint ('transformer_decoder') has no tokenizer and tokenizer.pth is never opened."""
+    from ._lib import ThmrError
     from .engine import TokenHMREngine
     ck = Path(checkpoint_path)
     root = ck.parent.parent if ck.parent.name == "checkpoints" else ck.parent
-    tokenizer_path = tokenizer_path or str(ck.parent / "tokenizer.pth")
     smpl_model_path = smpl_model_path or str(root / "body_models" / "smpl")
     if joint_regressor_extra is None and (root / "body_models" / "SMPL_to_J19.pkl").exists():
         joint_regressor_extra = str(root / "body_models" / "SMPL_to_J19.pkl")
-    net, arch = load_tokenizer_checkpoint(tokenizer_path)
-    cfg = config_from_files(model_cfg, arch)
-    sd = merge_state_dicts(load_lightning_state_dict(checkpoint_path), net)
+    model_sd = load_lightning_state_dict(checkpoint_path)
+    head = infer_head(model_sd)
+    yaml_head = config_from_files(model_cfg, head=head).head if model_cfg else head
+    if yaml_head != head:
+        raise ThmrError(f"{model_cfg} says MODEL.SMPL_HEAD.TYPE {yaml_head!r} but the checkpoint {checkpoint_path} holds "
+                        f"a {head!r} head")
+    net, arch = {}, None
+    if head == "token":
+        net, arch = load_tokenizer_checkpoint(tokenizer_path or str(ck.parent / "tokenizer.pth"))
+    cfg = config_from_files(model_cfg, arch, head=head)
+    sd = merge_state_dicts(model_sd, net)
     smpl = load_smpl_pkl(smpl_model_path, joint_regressor_extra, num_betas=cfg.num_betas)
     # what the files themselves imply: number of ViT blocks, mesh size
     import dataclasses

@@ -5,6 +5,7 @@ Mirrors the keys the reference reads at construction time (SURVEY.md §8 header)
   decoder    tokenhmr/lib/configs_hydra/experiment/tokenhmr_release.yaml:73-81, heads/token_head.py:30-38
   classifier heads/token_classifier.py:56-63, tokenhmr_release.yaml:69-72
   tokenizer  tokenization/configs/tokenizer_amass_moyo.yaml:41-53, models/vanilla_pose_vqvae.py:258-293
+  regression head  heads/smpl_head.py:14-34 (MODEL.SMPL_HEAD.TYPE: transformer_decoder)
   SMPL       tokenhmr_release.yaml:31-37;  EXTRA.FOCAL_LENGTH / MODEL.IMAGE_SIZE default.yaml:12, release:57
 """
 from __future__ import annotations
@@ -13,6 +14,9 @@ from dataclasses import asdict, dataclass
 from typing import List
 
 import numpy as np
+
+
+HEADS = ("token", "transformer_decoder")
 
 
 @dataclass(frozen=True)
@@ -55,6 +59,15 @@ class TokenHMRConfig:
     num_joints: int = 24
     num_betas: int = 10
     focal_length: float = 5000.0
+    # --- SMPL head (MODEL.SMPL_HEAD.TYPE, heads/__init__.py:4-13): "token" (SMPLTokenDecoderHead: token classifier +
+    # tokenizer decoder) or "transformer_decoder" (SMPLTransformerDecoderHead, HMR 2.0's regression head: decpose /
+    # decshape / deccam read the decoder's output token directly, smpl_head.py:32-34,82-84; no token classifier, no
+    # tokenizer, no cls_logits_softmax)
+    head: str = "token"
+
+    def __post_init__(self):
+        if self.head not in HEADS:
+            raise ValueError(f"TokenHMRConfig.head = {self.head!r}; one of {HEADS}")
 
     # derived ------------------------------------------------------------------------------------
     @property
@@ -100,9 +113,9 @@ def release_config() -> TokenHMRConfig:
     return TokenHMRConfig()
 
 
-def tiny_config(vit_depth: int = 2, num_verts: int = 431) -> TokenHMRConfig:
+def tiny_config(vit_depth: int = 2, num_verts: int = 431, head: str = "token") -> TokenHMRConfig:
     """Same layer shapes, fewer ViT blocks / SMPL vertices: for CPU-speed tests."""
-    return TokenHMRConfig(vit_depth=vit_depth, num_verts=num_verts)
+    return TokenHMRConfig(vit_depth=vit_depth, num_verts=num_verts, head=head)
 
 
 # SMPL kinematic tree (smplx body_models, SMPL: 24 joints)

@@ -133,6 +133,7 @@ inline int smpl_run(const thmr_smpl* sm, const float* pose, int pose2rot, const 
 
 struct thmr_engine {
   thmr_config cfg;
+  int head = THMR_HEAD_TOKEN;   // THMR_HEAD_TOKEN / THMR_HEAD_REGRESSION (thmr_engine_create_head)
   thmr_weights w;
   std::vector<thmr_vit_block> blocks;
   std::vector<thmr_vit_block_scales> block_scales;   // fp8 mode only
@@ -150,10 +151,12 @@ struct thmr_engine {
 namespace thmr {
 
 constexpr int kTokPad = 3;  // zero rows on both ends of every tokenizer-decoder sequence (max dilation)
+// regression head read-out rows: decpose (24 x 6) | decshape (10) | deccam (3) | 3 zero rows (a multiple of 32)
+constexpr int kRegReadoutRows = 160;
 
-// The forward's last step, the same in every mode: read-out assembly, 6D -> rotation (token_head.py:103-128), SMPL +
-// projection (tokenhmr.py:162-187).  carve() takes the buffers that stand in for the outputs a caller leaves null and
-// the SMPL workspace; push() plans the blend GEMM of every kSmplChunk-pose chunk and appends the step.
+// The forward's last step, the same in every mode and for both heads: read-out assembly, 6D -> rotation
+// (token_head.py:103-128, smpl_head.py:82-105), SMPL + projection (tokenhmr.py:162-187).  carve() takes the buffers
+// that stand in for the outputs a caller leaves null and the SMPL workspace; push() plans the blend GEMM of every kSmplChunk-pose chunk and appends the step.
 struct SmplTail {
   float *rot, *betas, *cam, *camt, *focal, *kp3, *kp2, *verts;
   SmplWs ws;
@@ -171,8 +174,11 @@ struct SmplTail {
     smpl_carve(bp, m, B, &ws);
   }
 
-  // readout: [B, 32] read-out GEMM output; out6: [B, Lpj, 8] 6D rotations with kTokPad pad rows either side
-  int push(StepList& S, const thmr_engine* e, int B, const float* readout, const float* out6, int Lpj) const {
+  // readout: [B, ld_r] read-out GEMM output.  Token head: out6 [B, pitch, ld6] holds the tokenizer decoder's 6D
+  // rotations of the 21 body joints with kTokPad pad rows either side.  Regression head: out6 is NULL and the read-out
+  // holds all 24 rotations (head_assemble_kernel).
+  int push(StepList& S, const thmr_engine* e, int B, const float* readout, int ld_r, const float* out6, int ld6,
+           int pitch) const {
     const thmr_smpl* sm = e->smpl;
     int err = THMR_OK;
     std::vector<GemmPlan> blend((B + kSmplChunk - 1) / kSmplChunk);
@@ -189,8 +195,8 @@ struct SmplTail {
       float* rot = r.out.rotmats ? r.out.rotmats : fb.rot;
       float* bet = r.out.betas ? r.out.betas : fb.betas;
       float* cam = r.out.pred_cam ? r.out.pred_cam : fb.cam;
-      head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(readout, 32, out6, 8, Lpj, kTokPad, ip, ib, ic, rot,
-                                                                bet, cam, r.out.pose6d, B, nb);
+      head_assemble_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(readout, ld_r, out6, ld6, pitch, kTokPad, ip, ib, ic,
+                                                                rot, bet, cam, r.out.pose6d, B, nb);
       THMR_CUDA(cudaGetLastError());
       float* verts = r.out.pred_vertices ? r.out.pred_vertices : fb.verts;
       float* kp3 = r.out.pred_keypoints_3d ? r.out.pred_keypoints_3d : fb.kp3;
@@ -216,6 +222,8 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   const int gw = (c.crop_w + 2 * c.patch_pad - c.patch) / c.patch + 1;
   const int KP = 3 * c.patch * c.patch;
   const int PAD = kTokPad;
+  const bool reg = e->head == THMR_HEAD_REGRESSION;
+  const int NR = reg ? kRegReadoutRows : 32;   // read-out GEMM width
 
   // ---------------------------------------------------------------- workspace
   __half* a0 = bp.take<__half>(static_cast<size_t>(M) * KP);
@@ -233,28 +241,32 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   __half* att16 = bp.take<__half>(static_cast<size_t>(B) * inner);
   __half* hid16 = bp.take<__half>(static_cast<size_t>(B) * c.dec_mlp_dim);
   unsigned long long* stamps = bp.take<unsigned long long>(kMaxStamps);   // in-graph start stamps, one slot per step
-  float* readout = bp.take<float>(static_cast<size_t>(B) * 32);
-  float* mt32 = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* cx = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  __half* cx16 = bp.take<__half>(static_cast<size_t>(B) * TN * CH);
-  __half* yT16 = bp.take<__half>(static_cast<size_t>(B) * CH * TN);
-  __half* t1 = bp.take<__half>(static_cast<size_t>(B) * CH * c.cls_token_inter);
-  float* yT32 = bp.take<float>(static_cast<size_t>(B) * CH * TN);
-  float* xy = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  __half* z16 = bp.take<__half>(static_cast<size_t>(B) * TN * CH);
-  __half* c1 = bp.take<__half>(static_cast<size_t>(B) * TN * c.cls_hidden_inter);
-  float* mn32 = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  __half* mn16 = bp.take<__half>(static_cast<size_t>(B) * TN * CH);
-  float* logits = bp.take<float>(static_cast<size_t>(B) * TN * NC);
-  float* probs_fallback = bp.take<float>(static_cast<size_t>(B) * TN * NC);
+  float* readout = bp.take<float>(static_cast<size_t>(B) * NR);
+  // classifier and tokenizer-decoder buffers: token head only (a regression engine takes them from an empty arena, so
+  // they are NULL and its workspace does not hold them)
+  Bump none(nullptr);
+  Bump& hb = reg ? none : bp;
+  float* mt32 = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* cx = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  __half* cx16 = hb.take<__half>(static_cast<size_t>(B) * TN * CH);
+  __half* yT16 = hb.take<__half>(static_cast<size_t>(B) * CH * TN);
+  __half* t1 = hb.take<__half>(static_cast<size_t>(B) * CH * c.cls_token_inter);
+  float* yT32 = hb.take<float>(static_cast<size_t>(B) * CH * TN);
+  float* xy = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  __half* z16 = hb.take<__half>(static_cast<size_t>(B) * TN * CH);
+  __half* c1 = hb.take<__half>(static_cast<size_t>(B) * TN * c.cls_hidden_inter);
+  float* mn32 = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  __half* mn16 = hb.take<__half>(static_cast<size_t>(B) * TN * CH);
+  float* logits = hb.take<float>(static_cast<size_t>(B) * TN * NC);
+  float* probs_fallback = hb.take<float>(static_cast<size_t>(B) * TN * NC);
   const int Lp0 = TN + 2 * PAD;
-  __half* p16 = bp.take<__half>(static_cast<size_t>(B) * Lp0 * NC);
-  __half* d16 = bp.take<__half>(static_cast<size_t>(B) * Lp0 * c.code_dim);
-  __half* bufA = bp.take<__half>(static_cast<size_t>(B) * Lp0 * W);
-  __half* bufB = bp.take<__half>(static_cast<size_t>(B) * Lp0 * W);
+  __half* p16 = hb.take<__half>(static_cast<size_t>(B) * Lp0 * NC);
+  __half* d16 = hb.take<__half>(static_cast<size_t>(B) * Lp0 * c.code_dim);
+  __half* bufA = hb.take<__half>(static_cast<size_t>(B) * Lp0 * W);
+  __half* bufB = hb.take<__half>(static_cast<size_t>(B) * Lp0 * W);
   const int Lj = c.tok_joints, Lpj = Lj + 2 * PAD;
-  float* x32 = bp.take<float>(static_cast<size_t>(B) * Lpj * W);
-  float* out6 = bp.take<float>(static_cast<size_t>(B) * Lpj * 8);
+  float* x32 = hb.take<float>(static_cast<size_t>(B) * Lpj * W);
+  float* out6 = hb.take<float>(static_cast<size_t>(B) * Lpj * 8);
   SmplTail tail;
   tail.carve(bp, e->smpl->m, B);
   // fp8 mode: xn and h hold e4m3 codes inside their fp16 buffers; their power-of-two scales are k-block-major
@@ -431,6 +443,18 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
     THMR_CUDA(cudaGetLastError());
     return THMR_OK;
   });
+  if (reg) {
+    // ---- regression head (smpl_head.py:82-84): decpose | decshape | deccam in one GEMM, then the SMPL tail
+    S.tag("head.readout_gemm");
+    linear(y16, E, B, w.readout_w, NR, E, w.readout_b, kActNone, readout, nullptr);
+    if (const int s = tail.push(S, e, B, readout, NR, nullptr, 0, 0); s != THMR_OK) err = s;
+    *status = err;
+    if (err == THMR_OK) {
+      const cudaError_t ce = cudaMemsetAsync(stamps, 0, kMaxStamps * sizeof(unsigned long long), stream);
+      if (ce != cudaSuccess) *status = fail(THMR_ERR_CUDA, "cudaMemsetAsync(flags): %s", cudaGetErrorString(ce));
+    }
+    return total;
+  }
   // read-outs: decpose_grot | decpose_hands | decshape | deccam (token_head.py:99-105) in one GEMM
   linear(y16, E, B, w.readout_w, 32, E, w.readout_b, kActNone, readout, nullptr);
 
@@ -513,7 +537,7 @@ inline size_t engine_build(thmr_engine* e, void* workspace, int B, bool build, i
   conv(bufA, Lcur, W, w.conv_post, W, 1, 3, kActNone, 0, nullptr, 0, bufB, nullptr);
   conv(bufB, Lcur, W, w.conv_out, 6, 1, 3, kActNone, 0, out6, 8, nullptr, nullptr);
 
-  if (const int s = tail.push(S, e, B, readout, out6, Lpj); s != THMR_OK) err = s;
+  if (const int s = tail.push(S, e, B, readout, 32, out6, 8, Lpj); s != THMR_OK) err = s;
   *status = err;
   // zero the padded fp16 probability buffer once (pad rows are never written afterwards)
   if (err == THMR_OK) {

@@ -26,6 +26,8 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   const int HID = c.vit_mlp_ratio * D;
   const int Lp0 = TN + 2 * PAD;
   const int Lj = c.tok_joints, Lpj = Lj + 2 * PAD;
+  const bool reg = e->head == THMR_HEAD_REGRESSION;
+  const int NR = reg ? kRegReadoutRows : 32;   // read-out GEMM width
 
   // ---------------------------------------------------------------- workspace (all activations fp32)
   // split-operand scratch: the widest A' of the forward
@@ -51,23 +53,26 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   float* q32 = bp.take<float>(static_cast<size_t>(B) * inner);
   float* att32 = bp.take<float>(static_cast<size_t>(B) * inner);
   float* hid32 = bp.take<float>(static_cast<size_t>(B) * c.dec_mlp_dim);
-  float* readout = bp.take<float>(static_cast<size_t>(B) * 32);
-  float* mt32 = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* cx = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* yT = bp.take<float>(static_cast<size_t>(B) * CH * TN);
-  float* t1 = bp.take<float>(static_cast<size_t>(B) * CH * c.cls_token_inter);
-  float* yT2 = bp.take<float>(static_cast<size_t>(B) * CH * TN);
-  float* xy = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* z32 = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* c1 = bp.take<float>(static_cast<size_t>(B) * TN * c.cls_hidden_inter);
-  float* mn32 = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* mnn = bp.take<float>(static_cast<size_t>(B) * TN * CH);
-  float* logits = bp.take<float>(static_cast<size_t>(B) * TN * NC);
-  float* probs_fallback = bp.take<float>(static_cast<size_t>(B) * TN * NC);
-  float* d32 = bp.take<float>(static_cast<size_t>(B) * Lp0 * c.code_dim);
-  float* bufA = bp.take<float>(static_cast<size_t>(B) * Lp0 * W);
-  float* bufB = bp.take<float>(static_cast<size_t>(B) * Lp0 * W);
-  float* out6 = bp.take<float>(static_cast<size_t>(B) * Lpj * 8);
+  float* readout = bp.take<float>(static_cast<size_t>(B) * NR);
+  // classifier and tokenizer-decoder buffers: token head only (NULL, and not in the workspace, for a regression engine)
+  Bump none(nullptr);
+  Bump& hb = reg ? none : bp;
+  float* mt32 = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* cx = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* yT = hb.take<float>(static_cast<size_t>(B) * CH * TN);
+  float* t1 = hb.take<float>(static_cast<size_t>(B) * CH * c.cls_token_inter);
+  float* yT2 = hb.take<float>(static_cast<size_t>(B) * CH * TN);
+  float* xy = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* z32 = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* c1 = hb.take<float>(static_cast<size_t>(B) * TN * c.cls_hidden_inter);
+  float* mn32 = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* mnn = hb.take<float>(static_cast<size_t>(B) * TN * CH);
+  float* logits = hb.take<float>(static_cast<size_t>(B) * TN * NC);
+  float* probs_fallback = hb.take<float>(static_cast<size_t>(B) * TN * NC);
+  float* d32 = hb.take<float>(static_cast<size_t>(B) * Lp0 * c.code_dim);
+  float* bufA = hb.take<float>(static_cast<size_t>(B) * Lp0 * W);
+  float* bufB = hb.take<float>(static_cast<size_t>(B) * Lp0 * W);
+  float* out6 = hb.take<float>(static_cast<size_t>(B) * Lpj * 8);
   SmplTail tail;
   tail.carve(bp, e->smpl->m, B);
   const size_t total = (bp.off + 1023) & ~size_t(1023);
@@ -214,6 +219,14 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
       THMR_CUDA(cudaMemcpyAsync(r.out.token_out, tok, sizeof(float) * B * E, cudaMemcpyDeviceToDevice, st));
     return THMR_OK;
   }, 0);
+  if (reg) {
+    // ---- regression head (smpl_head.py:82-84): decpose | decshape | deccam in one split-fp16 GEMM, then the SMPL tail
+    S.tag("head.readout_gemm");
+    lin(tok, E, B, kSplitActNone, w.readout_w, NR, w.readout_b, readout);
+    if (const int s = tail.push(S, e, B, readout, NR, nullptr, 0, 0); s != THMR_OK) err = s;
+    *status = err;
+    return total;
+  }
   lin(tok, E, B, kSplitActNone, w.readout_w, 32, w.readout_b, readout);
 
   // ---- token classifier (token_classifier.py:89-104)
@@ -305,7 +318,7 @@ inline size_t engine_build_strict(thmr_engine* e, void* workspace, int B, bool b
   conv(xres, Lcur, W, kSplitActNone, w.conv_post, W, 1, 3, bufB, W, nullptr);
   conv(bufB, Lcur, W, kSplitActNone, w.conv_out, 6, 1, 3, out6, 8, nullptr);
 
-  if (const int s = tail.push(S, e, B, readout, out6, Lpj); s != THMR_OK) err = s;
+  if (const int s = tail.push(S, e, B, readout, 32, out6, 8, Lpj); s != THMR_OK) err = s;
   *status = err;
   return total;
 }

@@ -1,4 +1,4 @@
-// Small per-image kernels of the SMPL token head: one-query cross-attention and the read-out assembly.
+// Small per-image kernels of the SMPL heads: one-query cross-attention and the read-out assembly.
 #pragma once
 #include "common.cuh"
 #include "elementwise.cuh"
@@ -70,10 +70,31 @@ dec_cross_attn_kernel(const float* __restrict__ q, const __half* __restrict__ kv
   }
 }
 
-// Read-out assembly (token_head.py:99-105,123-128) + rot6d_to_rotmat (geometry.py:64-84).
-//   readout (B, ld_r) fp32 = [grot(6) | hands(12) | betas(10) | cam(3)] linear outputs (bias included)
-//   bpose   rows (b*pitch + lo + j), 6 floats each: tokenizer decoder output for the 21 body joints
-//   pose6d = cat[grot, bpose(126), hands] + init_pose;  betas += init_betas;  cam += init_cam
+// rot6d_to_rotmat (geometry.py:64-84) of one 6D vector: x.reshape(2,3).permute -> a1 = x[0:3], a2 = x[3:6];
+// F.normalize eps = 1e-12; R rows b1, b2, b3 = b1 x b2.  The one copy of this arithmetic: the read-out assembly of
+// both heads and the stand-alone operator call it.
+__device__ __forceinline__ void rot6d_to_rotmat_one(const float* x, float* R) {
+  const float n1 = fmaxf(sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]), 1e-12f);
+  const float b1x = x[0] / n1, b1y = x[1] / n1, b1z = x[2] / n1;
+  const float dp = b1x * x[3] + b1y * x[4] + b1z * x[5];
+  const float ux = x[3] - dp * b1x, uy = x[4] - dp * b1y, uz = x[5] - dp * b1z;
+  const float n2 = fmaxf(sqrtf(ux * ux + uy * uy + uz * uz), 1e-12f);
+  const float b2x = ux / n2, b2y = uy / n2, b2z = uz / n2;
+  R[0] = b1x; R[1] = b1y; R[2] = b1z;
+  R[3] = b2x; R[4] = b2y; R[5] = b2z;
+  R[6] = b1y * b2z - b1z * b2y;
+  R[7] = b1z * b2x - b1x * b2z;
+  R[8] = b1x * b2y - b1y * b2x;
+}
+
+// Read-out assembly + rot6d_to_rotmat, for both SMPL heads.
+//   token head (bpose != NULL; token_head.py:99-105,123-128):
+//     readout (B, ld_r) fp32 = [grot(6) | hands(12) | betas(10) | cam(3)] linear outputs (bias included)
+//     bpose   rows (b*pitch + lo + j), 6 floats each: tokenizer decoder output for the 21 body joints
+//     pose6d = cat[grot, bpose(126), hands] + init_pose
+//   regression head (bpose == NULL; smpl_head.py:82-84,89-105):
+//     readout (B, ld_r) fp32 = [pose(144) | betas(10) | cam(3)];  pose6d = pose + init_pose
+//   both: betas += init_betas;  cam += init_cam
 // One thread per (image, joint).
 __global__ void head_assemble_kernel(const float* __restrict__ readout, int ld_r, const float* __restrict__ bpose,
                                      int ld_b, int pitch, int lo, const float* __restrict__ init_pose,
@@ -85,7 +106,10 @@ __global__ void head_assemble_kernel(const float* __restrict__ readout, int ld_r
   const int b = t / 24, j = t % 24;
   const float* r = readout + static_cast<size_t>(b) * ld_r;
   float x[6];
-  if (j == 0) {
+  if (!bpose) {
+#pragma unroll
+    for (int e = 0; e < 6; ++e) x[e] = r[j * 6 + e];
+  } else if (j == 0) {
 #pragma unroll
     for (int e = 0; e < 6; ++e) x[e] = r[e];
   } else if (j <= 21) {
@@ -102,22 +126,11 @@ __global__ void head_assemble_kernel(const float* __restrict__ readout, int ld_r
 #pragma unroll
     for (int e = 0; e < 6; ++e) pose6d_out[static_cast<size_t>(b) * 144 + j * 6 + e] = x[e];
   }
-  // x.reshape(2,3).permute -> a1 = x[0:3], a2 = x[3:6]; F.normalize eps = 1e-12
-  const float n1 = fmaxf(sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]), 1e-12f);
-  const float b1x = x[0] / n1, b1y = x[1] / n1, b1z = x[2] / n1;
-  const float dp = b1x * x[3] + b1y * x[4] + b1z * x[5];
-  const float ux = x[3] - dp * b1x, uy = x[4] - dp * b1y, uz = x[5] - dp * b1z;
-  const float n2 = fmaxf(sqrtf(ux * ux + uy * uy + uz * uz), 1e-12f);
-  const float b2x = ux / n2, b2y = uy / n2, b2z = uz / n2;
-  float* R = rotmats + static_cast<size_t>(t) * 9;
-  R[0] = b1x; R[1] = b1y; R[2] = b1z;
-  R[3] = b2x; R[4] = b2y; R[5] = b2z;
-  R[6] = b1y * b2z - b1z * b2y;
-  R[7] = b1z * b2x - b1x * b2z;
-  R[8] = b1x * b2y - b1y * b2x;
+  rot6d_to_rotmat_one(x, rotmats + static_cast<size_t>(t) * 9);
   if (j == 0) {
-    for (int l = 0; l < nb; ++l) betas[static_cast<size_t>(b) * nb + l] = r[18 + l] + init_betas[l];
-    for (int e = 0; e < 3; ++e) cam[b * 3 + e] = r[28 + e] + init_cam[e];
+    const int rb = bpose ? 18 : 144;   // first betas column of the read-out
+    for (int l = 0; l < nb; ++l) betas[static_cast<size_t>(b) * nb + l] = r[rb + l] + init_betas[l];
+    for (int e = 0; e < 3; ++e) cam[b * 3 + e] = r[rb + 10 + e] + init_cam[e];
   }
 }
 
@@ -125,19 +138,7 @@ __global__ void head_assemble_kernel(const float* __restrict__ readout, int ld_r
 __global__ void rot6d_kernel(const float* __restrict__ x6, float* __restrict__ rot, long N) {
   const long t = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
   if (t >= N) return;
-  const float* x = x6 + t * 6;
-  const float n1 = fmaxf(sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]), 1e-12f);
-  const float b1x = x[0] / n1, b1y = x[1] / n1, b1z = x[2] / n1;
-  const float dp = b1x * x[3] + b1y * x[4] + b1z * x[5];
-  const float ux = x[3] - dp * b1x, uy = x[4] - dp * b1y, uz = x[5] - dp * b1z;
-  const float n2 = fmaxf(sqrtf(ux * ux + uy * uy + uz * uz), 1e-12f);
-  const float b2x = ux / n2, b2y = uy / n2, b2z = uz / n2;
-  float* R = rot + t * 9;
-  R[0] = b1x; R[1] = b1y; R[2] = b1z;
-  R[3] = b2x; R[4] = b2y; R[5] = b2z;
-  R[6] = b1y * b2z - b1z * b2y;
-  R[7] = b1z * b2x - b1x * b2z;
-  R[8] = b1x * b2y - b1y * b2x;
+  rot6d_to_rotmat_one(x6 + t * 6, rot + t * 9);
 }
 
 }  // namespace thmr

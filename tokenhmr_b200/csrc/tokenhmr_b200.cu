@@ -911,6 +911,11 @@ int thmr_tokenhmr_loss(const thmr_loss_desc* d, void* workspace, void* stream) {
 
 // ------------------------------------------------------------------------------------------ engine
 int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr_smpl* smpl, thmr_engine** out) {
+  return thmr_engine_create_head(cfg, THMR_HEAD_TOKEN, w, smpl, out);
+}
+
+int thmr_engine_create_head(const thmr_config* cfg, int head_type, const thmr_weights* w, const thmr_smpl* smpl,
+                            thmr_engine** out) {
   THMR_CHECK(cfg && w && smpl && out, "engine_create: null argument");
   THMR_CHECK(cfg->vit_dim == cfg->vit_heads * kAttHeadDim, "engine_create: head_dim must be %d", kAttHeadDim);
   const int gh = (cfg->image_size + 2 * cfg->patch_pad - cfg->patch) / cfg->patch + 1;
@@ -927,7 +932,15 @@ int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr
   for (int k = 0; k < cfg->tok_depth - 1; ++k) maxdil *= cfg->tok_dilation_rate;
   THMR_CHECK(maxdil <= kTokPad, "engine_create: dilation %d exceeds sequence padding %d", maxdil, kTokPad);
   THMR_CHECK(smpl->m.nb <= 10 && smpl->m.n_extra + 25 <= 64, "engine_create: SMPL model shape");
-  THMR_CHECK(w->blocks_host && w->dec_host && w->mixer_host, "engine_create: missing layer arrays");
+  THMR_CHECK(head_type == THMR_HEAD_TOKEN || head_type == THMR_HEAD_REGRESSION,
+             "engine_create: head_type %d (THMR_HEAD_TOKEN or THMR_HEAD_REGRESSION)", head_type);
+  const bool token_head = head_type == THMR_HEAD_TOKEN;
+  THMR_CHECK(w->blocks_host && w->dec_host && (w->mixer_host || !token_head), "engine_create: missing layer arrays");
+  // readout_w: [32, E] for the token head, [160, E] (all 24 rotations, betas, camera) for the regression head
+  THMR_CHECK(w->readout_w && w->readout_b && w->init_pose && w->init_betas && w->init_cam,
+             "engine_create: missing %s read-out weights or mean parameters", token_head ? "token-head" : "regression-head");
+  THMR_CHECK(!token_head || (w->mt_w && w->cls_w && w->codebook_t && w->conv_out.w),
+             "engine_create: the token head needs the classifier and tokenizer weights");
   THMR_CHECK(!(cfg->strict && cfg->fp8), "engine_create: strict and fp8 are exclusive numeric modes");
   THMR_CHECK(!cfg->fp8 || w->block_scales_host, "engine_create: fp8 needs the weights' block scales");
   THMR_CHECK(!cfg->fp8 || (cfg->vit_dim % 128 == 0 && (cfg->vit_dim == 1280 || cfg->vit_dim == 1024 ||
@@ -936,11 +949,12 @@ int thmr_engine_create(const thmr_config* cfg, const thmr_weights* w, const thmr
   thmr_engine* e = new (std::nothrow) thmr_engine();
   if (!e) return fail(THMR_ERR_NOMEM, "engine_create: out of host memory");
   e->cfg = *cfg;
+  e->head = head_type;
   e->w = *w;
   e->blocks.assign(w->blocks_host, w->blocks_host + cfg->vit_depth);
   if (cfg->fp8) e->block_scales.assign(w->block_scales_host, w->block_scales_host + cfg->vit_depth);
   e->dec.assign(w->dec_host, w->dec_host + cfg->dec_depth);
-  e->mixer.assign(w->mixer_host, w->mixer_host + cfg->cls_blocks);
+  if (token_head) e->mixer.assign(w->mixer_host, w->mixer_host + cfg->cls_blocks);
   e->w.blocks_host = nullptr; e->w.dec_host = nullptr; e->w.mixer_host = nullptr; e->w.block_scales_host = nullptr;
   e->smpl = smpl;
   *out = e;
@@ -975,9 +989,17 @@ static int engine_prepare(thmr_engine* e, int B, void* workspace, cudaStream_t s
   return THMR_OK;
 }
 
+// A regression engine has no token classifier: a caller who asks for its probabilities learns it before anything runs.
+static int check_outputs(const thmr_engine* e, const thmr_outputs* out) {
+  THMR_CHECK(!(e && e->head == THMR_HEAD_REGRESSION && out->cls_logits_softmax),
+             "engine_forward: a regression-head engine produces no cls_logits_softmax (its pointer must be NULL)");
+  return THMR_OK;
+}
+
 int thmr_engine_forward(thmr_engine* e, const float* img, int B, const thmr_outputs* out, void* workspace,
                         void* stream) {
   THMR_CHECK(img && out, "engine_forward: null argument");
+  THMR_TRY(check_outputs(e, out));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   THMR_TRY(engine_prepare(e, B, workspace, st));
   RunCtx ctx{img, *out, nullptr};
@@ -1024,6 +1046,7 @@ int thmr_engine_step_info(const thmr_engine* e, int i, const char** name, double
 int thmr_engine_profile(thmr_engine* e, const float* img, int B, const thmr_outputs* out, void* workspace, void* stream,
                         float* step_ms, int cap) {
   THMR_CHECK(img && out && step_ms, "engine_profile: null argument");
+  THMR_TRY(check_outputs(e, out));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   THMR_TRY(engine_prepare(e, B, workspace, st));
   const int n = static_cast<int>(e->steps.size());
@@ -1096,6 +1119,7 @@ int thmr_comm_rank(const thmr_comm* c) { return c ? c->rank : -1; }
 
 int thmr_allgather_outputs(const thmr_engine* e, thmr_comm* c, const thmr_outputs* g, int rows, void* stream) {
   THMR_CHECK(e && c && g && rows > 0, "allgather_outputs: bad argument");
+  THMR_TRY(check_outputs(e, g));
   NcclApi* api = nccl_api();
   THMR_CHECK(api && c->comm, "allgather_outputs: communicator not initialised");
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -23,6 +23,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.distributed as dist
 
+from . import _lib
+
 # (output key, per-image shape) in packing order; shapes are filled from the first output dict
 GATHER_KEYS = ["pred_vertices", "pred_keypoints_3d", "pred_keypoints_2d", "pred_cam", "pred_cam_t", "focal_length",
                "global_orient", "body_pose", "betas"]
@@ -116,6 +118,9 @@ class ShardedTokenHMR:
             raise ValueError("the native transport needs a TokenHMREngine")
         self.transport = transport
         self.gather_logits = bool(gather_logits)
+        if self.gather_logits and not getattr(model, "has_logits", True):
+            raise _lib.ThmrError("gather_logits=True: a regression-head (transformer_decoder) model produces no "
+                                 "cls_logits_softmax")
         self._comm = None
         self._sizes: Dict[int, List[int]] = {}
         self._send = None
@@ -207,6 +212,6 @@ class ShardedTokenHMR:
         res = _as_output_dict(trim(parts, spec.rows, sizes))
         if self.gather_logits:
             res["cls_logits_softmax"] = trim({"p": out["cls_logits_softmax"]}, spec.rows, sizes)["p"]
-        else:
+        elif "cls_logits_softmax" in out:
             res["cls_logits_softmax_local"] = out["cls_logits_softmax"]
         return res

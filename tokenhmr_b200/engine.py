@@ -78,7 +78,9 @@ class TokenHMREngine(nn.Module):
         (TokenHMRPipeline(streams=2)); the engine then avoids kernels that need the whole GPU to themselves
         (thmr_config::concurrent).
         fp8: the ViT's QKV, fc1 and fc2 GEMMs (88 % of the model's FLOPs) run on block-scaled e4m3 operands on the FP8
-        tensor cores (thmr_config::fp8, DESIGN.md §2 for its accuracy); not with strict."""
+        tensor cores (thmr_config::fp8, DESIGN.md §2 for its accuracy); not with strict.
+        cfg.head selects the SMPL head: "token" (TokenHMR) or "transformer_decoder" (HMR 2.0's regression head, whose
+        output dict has no cls_logits_softmax, as in the reference's forward_step, tokenhmr.py:157-158)."""
         if strict and fp8:
             raise _lib.ThmrError("strict and fp8 are exclusive numeric modes")
         super().__init__()
@@ -94,6 +96,7 @@ class TokenHMREngine(nn.Module):
         self.strict = bool(strict)
         self.concurrent = bool(concurrent)
         self.fp8 = bool(fp8)
+        self.has_logits = cfg.head == "token"     # the regression head has no token classifier
         self.alias_outputs = bool(alias_outputs)
         self.max_cached_shapes = int(max_cached_shapes)
         with torch.cuda.device(self.device):
@@ -103,8 +106,9 @@ class TokenHMREngine(nn.Module):
             self._cfg_struct = make_config_struct(cfg, strict=self.strict, concurrent=self.concurrent,
                                                   fp8=self.fp8)
             h = ctypes.c_void_p()
-            check(lib().thmr_engine_create(ctypes.byref(self._cfg_struct), ctypes.byref(self.weights.struct),
-                                           self.smpl_model.handle, ctypes.byref(h)))
+            head = _lib.HEAD_TOKEN if self.has_logits else _lib.HEAD_REGRESSION
+            check(lib().thmr_engine_create_head(ctypes.byref(self._cfg_struct), head, ctypes.byref(self.weights.struct),
+                                                self.smpl_model.handle, ctypes.byref(h)))
             self._h = h
         self.max_batch = max_batch
         self.use_cuda_graph = use_cuda_graph
@@ -159,6 +163,8 @@ class TokenHMREngine(nn.Module):
             raise _lib.ThmrError(f"batch of {B} images exceeds max_batch={self.max_batch} (raise it at construction)")
         if shard is not None and not (0 < B <= shard.rows and 0 <= shard.rank < shard.world):
             raise _lib.ThmrError(f"shard {shard} cannot hold a local batch of {B}")
+        if shard is not None and shard.gather_logits and not self.has_logits:
+            raise _lib.ThmrError("gather_logits: a regression-head engine produces no cls_logits_softmax")
         key = (B, int(taps), slot) + ((shard.world, shard.rank, shard.rows, shard.gather_logits) if shard else ())
         st = self._bufs.get(key)
         if st is not None:
@@ -175,7 +181,7 @@ class TokenHMREngine(nn.Module):
         f = lambda *s: torch.empty(*s, device=dev, dtype=torch.float32)
         t = {
             "img": f(B, 3, c.image_size, c.image_size),
-            "cls_logits_softmax": f(B, c.token_num, c.token_class_num),
+            **({"cls_logits_softmax": f(B, c.token_num, c.token_class_num)} if self.has_logits else {}),
             "pred_cam": f(B, 3), "rotmats": f(B, c.num_joints, 3, 3), "betas": f(B, c.num_betas),
             "pred_cam_t": f(B, 3), "focal_length": f(B, 2), "pred_keypoints_3d": f(B, nj, 3),
             "pred_vertices": f(B, self.smpl_model.num_verts, 3), "pred_keypoints_2d": f(B, nj, 2),
@@ -247,7 +253,7 @@ class TokenHMREngine(nn.Module):
                 t.update(st["g"])           # gathered fields: all world * rows images
             rot = t["rotmats"]
             out = {
-                "cls_logits_softmax": t["cls_logits_softmax"],
+                **({"cls_logits_softmax": t["cls_logits_softmax"]} if self.has_logits else {}),
                 "pred_cam": t["pred_cam"],
                 "pred_smpl_params": {"global_orient": rot[:, :1].clone(), "body_pose": rot[:, 1:].clone(),
                                      "betas": t["betas"].clone()},

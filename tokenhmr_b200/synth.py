@@ -8,6 +8,7 @@ packer (tokenhmr_b200/weights.py):
   backbone.*    ViT             tokenhmr/lib/models/backbones/vit.py:209-255
   smpl_head.*   token head      tokenhmr/lib/models/heads/token_head.py:20-63, token_classifier.py:52-86,
                                 components/pose_transformer.py:160-201,301-347
+                or, with cfg.head == "transformer_decoder", the regression head  heads/smpl_head.py:14-50
   tokenizer.*   'net' dict of tokenizer.pth: decoder.* / quantizer.codebook
                                 tokenization/models/vanilla_pose_vqvae.py:113-154, quantize_cnn.py:14-18
   smpl.*        body-model buffers of smplx.SMPLLayer + joint_regressor_extra (smpl_wrapper.py:11-25)
@@ -64,7 +65,8 @@ class _Maker:
 
 
 def make_state_dict(cfg: TokenHMRConfig, seed: int = 1234) -> Dict[str, torch.Tensor]:
-    """Synthetic fp32 parameters for backbone.*, smpl_head.* and tokenizer.* (CPU tensors)."""
+    """Synthetic fp32 parameters for backbone.*, smpl_head.* and tokenizer.* (CPU tensors).  The regression head
+    (cfg.head == "transformer_decoder") has the same backbone.* and smpl_head.transformer.* tensors and no tokenizer."""
     m = _Maker(seed)
     D = cfg.vit_dim
     # ---- ViT (vit.py:240-255)
@@ -99,15 +101,20 @@ def make_state_dict(cfg: TokenHMRConfig, seed: int = 1234) -> Dict[str, torch.Te
         m.layernorm(p + ".2.norm", E)
         m.linear(p + ".2.fn.net.0", cfg.dec_mlp_dim, E)
         m.linear(p + ".2.fn.net.3", E, cfg.dec_mlp_dim)
+    if cfg.head == "transformer_decoder":
+        # read-outs (smpl_head.py:32-34); the small decpose gain keeps all 24 rotations near the identity mean pose
+        # (well-conditioned 6D), as decpose_grot's does for the token head
+        m.linear("smpl_head.decpose", cfg.npose, E, gain=0.1)
+        m.linear("smpl_head.decshape", 10, E, gain=0.5)
+        m.linear("smpl_head.deccam", 3, E, gain=0.1)
+        _mean_params(m, cfg)
+        return m.sd
     # read-outs (token_head.py:40-43); small gain keeps the pose near the mean pose (well-conditioned 6D)
     m.linear("smpl_head.decpose_grot", 6, E, gain=0.3)
     m.linear("smpl_head.decshape", 10, E, gain=0.5)
     m.linear("smpl_head.deccam", 3, E, gain=0.1)
     m.linear("smpl_head.decpose_hands", 12, E, gain=0.3)
-    # mean params (token_head.py:57-63): identity 6D pose, zero shape, cam [0.9, 0, 0]
-    m.sd["smpl_head.init_body_pose"] = torch.tensor([1., 0., 0., 0., 1., 0.] * cfg.num_joints).view(1, -1)
-    m.sd["smpl_head.init_betas"] = torch.zeros(1, cfg.num_betas)
-    m.sd["smpl_head.init_cam"] = torch.tensor([[0.9, 0.0, 0.0]])
+    _mean_params(m, cfg)
 
     # ---- token classifier (token_classifier.py:67-80, modules.py)
     H = cfg.cls_hidden
@@ -141,6 +148,13 @@ def make_state_dict(cfg: TokenHMRConfig, seed: int = 1234) -> Dict[str, torch.Te
     m.conv1d(f"{t}.{idx + 1}", 6, W, 3)
     m.normal("tokenizer.quantizer.codebook", (cfg.nb_code, cfg.code_dim), 1.0)
     return m.sd
+
+
+def _mean_params(m: _Maker, cfg: TokenHMRConfig) -> None:
+    """Mean params (token_head.py:57-63, smpl_head.py:42-48): identity 6D pose, zero shape, cam [0.9, 0, 0]."""
+    m.sd["smpl_head.init_body_pose"] = torch.tensor([1., 0., 0., 0., 1., 0.] * cfg.num_joints).view(1, -1)
+    m.sd["smpl_head.init_betas"] = torch.zeros(1, cfg.num_betas)
+    m.sd["smpl_head.init_cam"] = torch.tensor([[0.9, 0.0, 0.0]])
 
 
 def make_tokenizer_encoder_state_dict(cfg: TokenHMRConfig, seed: int = 1234) -> Dict[str, torch.Tensor]:

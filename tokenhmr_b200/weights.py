@@ -2,7 +2,8 @@
 
 Accepts the key names of the reference checkpoints:
   * TokenHMR Lightning checkpoint ckpt['state_dict'] with prefixes 'backbone.' / 'smpl_head.'
-    (tokenhmr/lib/utils/misc.py:215-256 prepare_statedict / load_pretrained),
+    (tokenhmr/lib/utils/misc.py:215-256 prepare_statedict / load_pretrained); with cfg.head == "transformer_decoder"
+    the HMR 2.0 checkpoint's head (heads/smpl_head.py:14-50: transformer.*, decpose, decshape, deccam, init_*),
   * tokenizer.pth {'net': {'decoder.*', 'quantizer.codebook', ...}, 'hparams': ...} under the prefix
     'tokenizer.' (tokenization/models/vanilla_pose_vqvae.py:24-40,299-301; 'body_model' keys skipped),
 and produces fp16 [out,in] matrices / fp32 vectors on the GPU plus the ctypes thmr_weights struct.
@@ -69,7 +70,11 @@ class PackedWeights:
         self.strict = bool(strict)
         self.fp8 = bool(fp8)
         self._keep: List[torch.Tensor] = []
-        g = lambda n: sd[n]
+        self.keys_read: List[str] = []     # every state-dict entry the packer used, in order
+
+        def g(n: str) -> torch.Tensor:
+            self.keys_read.append(n)
+            return sd[n]
 
         def f16(t: torch.Tensor, taps: int = 1) -> int:
             if self.strict:
@@ -124,6 +129,11 @@ class PackedWeights:
         # ---- decoder
         t = "smpl_head.transformer."
         inner = cfg.dec_inner
+        # to_token_embedding(zeros(B, 1, 1)) = its bias: the weight multiplies the zero query token (token_head.py:91,
+        # smpl_head.py:75); a (E, npose + 13) weight would be TRANSFORMER_INPUT='mean_shape', which is not implemented
+        if g(t + "to_token_embedding.weight").shape[1] != 1:
+            raise _lib.ThmrError("to_token_embedding takes more than one input: a TRANSFORMER_INPUT='mean_shape' "
+                                 "checkpoint is not supported")
         W.token0 = f32(g(t + "to_token_embedding.bias") + g(t + "pos_embedding")[0, 0])
         W.kv_w = f16(torch.cat([g(f"{t}transformer.layers.{l}.1.fn.to_kv.weight") for l in range(cfg.dec_depth)], 0))
         self.dec = (_lib.DecLayer * cfg.dec_depth)()
@@ -141,14 +151,25 @@ class PackedWeights:
             d.ff2_w, d.ff2_b = f16(g(p + "2.fn.net.3.weight")), f32(g(p + "2.fn.net.3.bias"))
         W.dec_host = ctypes.cast(self.dec, ctypes.POINTER(_lib.DecLayer))
         h = "smpl_head."
-        order = ["decpose_grot", "decpose_hands", "decshape", "deccam"]   # 6 | 12 | 10 | 3 (+1 zero row)
-        rw = torch.cat([g(h + n + ".weight") for n in order] + [torch.zeros(1, cfg.dec_dim)], 0)
-        rb = torch.cat([g(h + n + ".bias") for n in order] + [torch.zeros(1)], 0)
-        assert rw.shape[0] == 32
+        regression = cfg.head == "transformer_decoder"
+        if regression:
+            order, rows = ["decpose", "decshape", "deccam"], 160            # 144 | 10 | 3 (+3 zero rows)
+        else:
+            order, rows = ["decpose_grot", "decpose_hands", "decshape", "deccam"], 32   # 6 | 12 | 10 | 3 (+1 zero row)
+        rw = torch.cat([g(h + n + ".weight") for n in order], 0)
+        rb = torch.cat([g(h + n + ".bias") for n in order], 0)
+        pad = rows - rw.shape[0]
+        rw = torch.cat([rw, torch.zeros(pad, cfg.dec_dim)], 0)
+        rb = torch.cat([rb, torch.zeros(pad)], 0)
         W.readout_w, W.readout_b = f16(rw), f32(rb)
         W.init_pose = f32(g(h + "init_body_pose").reshape(-1))
         W.init_betas = f32(g(h + "init_betas").reshape(-1))
         W.init_cam = f32(g(h + "init_cam").reshape(-1))
+        if regression:
+            # no classifier and no tokenizer: their pointers stay NULL (thmr_engine_create_head)
+            self.mixer = None
+            self.struct = W
+            return
         # ---- classifier
         c = h + "decpose."
         W.mt_w, W.mt_b = f16(g(c + "mixer_trans.ff.0.weight")), f32(g(c + "mixer_trans.ff.0.bias"))
