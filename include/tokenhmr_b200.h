@@ -284,6 +284,53 @@ size_t thmr_tokenhmr_loss_workspace_bytes(int B);
 int thmr_tokenhmr_loss(const thmr_loss_desc* desc, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training HMR 2.0's regression head (SMPLTransformerDecoderHead, heads/smpl_head.py:52-105 with IEF_ITERS 1,
+ * TRANSFORMER_INPUT 'zero', JOINT_REP '6d'): an fp32 forward that keeps its activations in the workspace, and the
+ * backward to every parameter.  Decoder width 1024, dim_head 64, context 1280 x 192 (the ViT-H features).
+ *
+ * Parameters and gradients live in flat fp32 buffers whose layout thmr_reg_head_param_info enumerates: the parameters
+ * of the reference head in named_parameters() order, under their state_dict names, each at a 64-float aligned offset.
+ * The three init_* mean parameters are buffers, passed separately.
+ *
+ * thmr_reg_head_backward reads the activations thmr_reg_head_train_forward left in the same workspace, with the same
+ * parameters.  It writes every gradient (exact zeros for the Q and K thirds of each self-attention to_qkv and for
+ * to_token_embedding.weight, whose input is zero), sums over the batch in a fixed order without atomics, and takes no
+ * gradient for the features.  Neither call synchronises the host; both can be captured in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct thmr_reg_head_desc {
+  int B;                        /* >= 1 */
+  int depth;                    /* 1 .. 64 decoder layers */
+  int heads;                    /* 1 .. 8 (dim_head 64) */
+  int mlp_dim;                  /* 1 .. 16384 */
+  const float* params;          /* flat parameters (thmr_reg_head_param_info layout) */
+  float* grads;                 /* flat gradients, same layout (backward only) */
+  const float* init_body_pose;  /* [144] */
+  const float* init_betas;      /* [10] */
+  const float* init_cam;        /* [3] */
+  const float* feats;           /* [B,1280,16,12] the backbone's channel-first features */
+  float* pose6d;                /* [B,144] output, may be NULL */
+  float* betas;                 /* [B,10] output */
+  float* cam;                   /* [B,3] output: pred_cam */
+  float* rotmats;               /* [B,24,3,3] output: global_orient, then body_pose */
+  const float* grad_pose6d;     /* upstream gradients for the backward, each may be NULL (zero): [B,144] */
+  const float* grad_betas;      /* [B,10] */
+  const float* grad_cam;        /* [B,3] */
+  const float* grad_rotmats;    /* [B,24,3,3] */
+  void* workspace;              /* thmr_reg_head_workspace_bytes(B, depth, heads, mlp_dim) bytes, 256-byte aligned */
+  size_t workspace_bytes;
+  void* stream;                 /* cudaStream_t */
+} thmr_reg_head_desc;
+/* Number of parameters and the floats of a flat buffer that holds them. */
+int thmr_reg_head_num_params(int depth, int heads, int mlp_dim, int* count, int64_t* total_floats);
+/* Parameter i: its state_dict name (valid until the next call on this thread), ndim, shape[0..ndim) and its offset in
+ * floats. */
+int thmr_reg_head_param_info(int depth, int heads, int mlp_dim, int i, const char** name, int* ndim, int64_t* shape,
+                             int64_t* offset);
+size_t thmr_reg_head_workspace_bytes(int B, int depth, int heads, int mlp_dim);
+int thmr_reg_head_train_forward(const thmr_reg_head_desc* desc);
+int thmr_reg_head_backward(const thmr_reg_head_desc* desc);
+
+/* ------------------------------------------------------------------------------------------------
  * Tokenizer encoder + hard quantisation (SURVEY §8 row f4): EncodeTokens
  * [tokenization/models/vanilla_pose_vqvae.py:304-346 -> PoseSPEncoderV1 :42-111, quantize_cnn.py:74-86]
  * ---------------------------------------------------------------------------------------------- */

@@ -47,6 +47,14 @@ class LossDesc(Structure):
                                         "grad_rotmats", "grad_betas")]
 
 
+class RegHeadDesc(Structure):
+    _fields_ = [("B", c_int), ("depth", c_int), ("heads", c_int), ("mlp_dim", c_int)] + \
+               [(n, c_void_p) for n in ("params", "grads", "init_body_pose", "init_betas", "init_cam", "feats", "pose6d",
+                                        "betas", "cam", "rotmats", "grad_pose6d", "grad_betas", "grad_cam",
+                                        "grad_rotmats", "workspace")] + \
+               [("workspace_bytes", c_size_t), ("stream", c_void_p)]
+
+
 class Config(Structure):
     _fields_ = [("image_size", c_int), ("crop_w", c_int), ("patch", c_int), ("patch_pad", c_int),
                 ("vit_dim", c_int), ("vit_depth", c_int), ("vit_heads", c_int), ("vit_mlp_ratio", c_int),
@@ -229,6 +237,12 @@ SIGNATURES = {
                                           c_void_p, c_void_p, c_void_p]),
     "thmr_tokenhmr_loss_workspace_bytes": (c_size_t, [c_int]),
     "thmr_tokenhmr_loss": (c_int, [POINTER(LossDesc), c_void_p, c_void_p]),
+    "thmr_reg_head_num_params": (c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
+    "thmr_reg_head_param_info": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_char_p), POINTER(c_int),
+                                         POINTER(c_int64), POINTER(c_int64)]),
+    "thmr_reg_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "thmr_reg_head_train_forward": (c_int, [POINTER(RegHeadDesc)]),
+    "thmr_reg_head_backward": (c_int, [POINTER(RegHeadDesc)]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_create_head": (c_int, [POINTER(Config), c_int, POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),

@@ -87,6 +87,45 @@ __device__ __forceinline__ void rot6d_to_rotmat_one(const float* x, float* R) {
   R[8] = b1x * b2y - b1y * b2x;
 }
 
+// Backward of rot6d_to_rotmat_one: x the 6D input, g = dL/dR (rows b1, b2, b3) -> gx = dL/dx.  b1 and b2 come from
+// the forward itself; the two norms are recovered as |a1| = a1 . b1 and |u| = a2 . b2 (b2 is orthogonal to b1).  A norm
+// at F.normalize's clamp (1e-12) is a constant, so its projection term drops.
+__device__ __forceinline__ void rot6d_to_rotmat_backward_one(const float* x, const float* g, float* gx) {
+  float R[9];
+  rot6d_to_rotmat_one(x, R);
+  const float* b1 = R;
+  const float* b2 = R + 3;
+  const float* g3 = g + 6;
+  const float r1 = x[0] * b1[0] + x[1] * b1[1] + x[2] * b1[2];
+  const float dp = x[3] * b1[0] + x[4] * b1[1] + x[5] * b1[2];
+  const float r2 = x[3] * b2[0] + x[4] * b2[1] + x[5] * b2[2];
+  const float n1 = fmaxf(r1, 1e-12f), n2 = fmaxf(r2, 1e-12f);
+  // b3 = b1 x b2:  dL/db1 += b2 x g3,  dL/db2 += g3 x b1
+  float gb1[3] = {g[0] + b2[1] * g3[2] - b2[2] * g3[1], g[1] + b2[2] * g3[0] - b2[0] * g3[2],
+                  g[2] + b2[0] * g3[1] - b2[1] * g3[0]};
+  const float gb2[3] = {g[3] + g3[1] * b1[2] - g3[2] * b1[1], g[4] + g3[2] * b1[0] - g3[0] * b1[2],
+                        g[5] + g3[0] * b1[1] - g3[1] * b1[0]};
+  // b2 = u / |u|
+  const float pb2 = r2 > 1e-12f ? b2[0] * gb2[0] + b2[1] * gb2[1] + b2[2] * gb2[2] : 0.f;
+  float gu[3], ga2[3];
+#pragma unroll
+  for (int e = 0; e < 3; ++e) gu[e] = (gb2[e] - pb2 * b2[e]) / n2;
+  // u = a2 - dp b1,  dp = b1 . a2
+  const float gdp = -(gu[0] * b1[0] + gu[1] * b1[1] + gu[2] * b1[2]);
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    ga2[e] = gu[e] + gdp * b1[e];
+    gb1[e] += -dp * gu[e] + gdp * x[3 + e];
+  }
+  // b1 = a1 / |a1|
+  const float pb1 = r1 > 1e-12f ? b1[0] * gb1[0] + b1[1] * gb1[1] + b1[2] * gb1[2] : 0.f;
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    gx[e] = (gb1[e] - pb1 * b1[e]) / n1;
+    gx[3 + e] = ga2[e];
+  }
+}
+
 // Read-out assembly + rot6d_to_rotmat, for both SMPL heads.
 //   token head (bpose != NULL; token_head.py:99-105,123-128):
 //     readout (B, ld_r) fp32 = [grot(6) | hands(12) | betas(10) | cam(3)] linear outputs (bias included)

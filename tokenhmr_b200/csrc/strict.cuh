@@ -29,6 +29,10 @@ enum : int { kSplitActNone = 0, kSplitActGelu = 1, kSplitActRelu = 2 };
 
 // nn.GELU() (approximate='none'): 0.5 x (1 + erf(x / sqrt(2))), erff = CUDA libm (<= 2 ulp)
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+// d gelu_exact / dx = Phi(x) + x phi(x)
+__device__ __forceinline__ float gelu_exact_grad(float x) {
+  return 0.5f * (1.0f + erff(x * 0.70710678118654752f)) + x * 0.39894228040143268f * expf(-0.5f * x * x);
+}
 
 // src fp32 [R, C] (row pitch lds) -> dst fp16 [*, 3C] = [hi | lo | hi] of act(x) * 2^4.
 // Optional row remap into zero-padded sequences: source row r = b*T + t  ->  dst row b*pitch + lo + t  (T == 0: identity).

@@ -8,6 +8,7 @@
 #include "engine.cuh"
 #include "engine_strict.cuh"
 #include "eval_kernels.cuh"
+#include "head_train.cuh"
 #include "keypoints.cuh"
 #include "losses.cuh"
 #include "preproc.cuh"
@@ -907,6 +908,76 @@ int thmr_tokenhmr_loss(const thmr_loss_desc* d, void* workspace, void* stream) {
                  (d->grad_rotmats != nullptr) + (d->grad_betas != nullptr);
   THMR_CHECK(ng == 0 || ng == 4, "tokenhmr_loss: the four gradient outputs must be all set or all NULL");
   return tokenhmr_loss_run(*d, workspace, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------ regression-head training
+static bool reg_head_dims_ok(int depth, int heads, int mlp_dim) {
+  return depth >= 1 && depth <= 64 && heads >= 1 && heads <= kRhMaxHeads && mlp_dim >= 1 && mlp_dim <= 16384;
+}
+
+int thmr_reg_head_num_params(int depth, int heads, int mlp_dim, int* count, int64_t* total_floats) {
+  THMR_CHECK(count && total_floats, "reg_head_num_params: null argument");
+  THMR_CHECK(reg_head_dims_ok(depth, heads, mlp_dim),
+             "reg_head: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)",
+             depth, heads, mlp_dim, kRhMaxHeads);
+  *count = rh_num_params(depth);
+  *total_floats = rh_param_floats(depth, heads, mlp_dim);
+  return THMR_OK;
+}
+
+int thmr_reg_head_param_info(int depth, int heads, int mlp_dim, int i, const char** name, int* ndim, int64_t* shape,
+                             int64_t* offset) {
+  static thread_local RhParam p;
+  THMR_CHECK(name && ndim && shape && offset, "reg_head_param_info: null argument");
+  THMR_CHECK(reg_head_dims_ok(depth, heads, mlp_dim),
+             "reg_head: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)",
+             depth, heads, mlp_dim, kRhMaxHeads);
+  THMR_CHECK(rh_param(depth, heads, mlp_dim, i, &p), "reg_head_param_info: index %d outside [0, %d)", i,
+             rh_num_params(depth));
+  *name = p.name;
+  *ndim = p.ndim;
+  for (int k = 0; k < p.ndim; ++k) shape[k] = p.shape[k];
+  *offset = p.offset;
+  return THMR_OK;
+}
+
+size_t thmr_reg_head_workspace_bytes(int B, int depth, int heads, int mlp_dim) {
+  if (B < 1 || !reg_head_dims_ok(depth, heads, mlp_dim)) return 0;
+  return rh_workspace_bytes(B, depth, heads, mlp_dim);
+}
+
+static int reg_head_check(const thmr_reg_head_desc* d, bool backward, RhWs* ws) {
+  const char* what = backward ? "reg_head_backward" : "reg_head_train_forward";
+  THMR_CHECK(d, "%s: null descriptor", what);
+  THMR_CHECK(d->B >= 1, "%s: B=%d (must be >= 1)", what, d->B);
+  THMR_CHECK(reg_head_dims_ok(d->depth, d->heads, d->mlp_dim),
+             "%s: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)", what,
+             d->depth, d->heads, d->mlp_dim, kRhMaxHeads);
+  THMR_CHECK(d->params && d->feats && d->init_body_pose && d->init_betas && d->init_cam, "%s: null input pointer",
+             what);
+  THMR_CHECK(d->workspace, "%s: null workspace", what);
+  THMR_CHECK((reinterpret_cast<uintptr_t>(d->workspace) & 255) == 0 && (reinterpret_cast<uintptr_t>(d->params) & 15) == 0 &&
+                 (!d->grads || (reinterpret_cast<uintptr_t>(d->grads) & 15) == 0),
+             "%s: workspace must be 256-byte and params / grads 16-byte aligned", what);
+  const size_t need = rh_workspace_bytes(d->B, d->depth, d->heads, d->mlp_dim);
+  THMR_CHECK(d->workspace_bytes >= need, "%s: workspace too small: %zu bytes, need %zu", what, d->workspace_bytes,
+             need);
+  if (backward) THMR_CHECK(d->grads, "%s: null gradient buffer", what);
+  else THMR_CHECK(d->betas && d->cam && d->rotmats, "%s: null output pointer", what);
+  rh_carve(static_cast<float*>(d->workspace), d->B, d->depth, d->heads, d->mlp_dim, ws);
+  return THMR_OK;
+}
+
+int thmr_reg_head_train_forward(const thmr_reg_head_desc* d) {
+  static thread_local RhWs ws;
+  THMR_TRY(reg_head_check(d, false, &ws));
+  return rh_forward(*d, ws, static_cast<cudaStream_t>(d->stream));
+}
+
+int thmr_reg_head_backward(const thmr_reg_head_desc* d) {
+  static thread_local RhWs ws;
+  THMR_TRY(reg_head_check(d, true, &ws));
+  return rh_backward(*d, ws, static_cast<cudaStream_t>(d->stream));
 }
 
 // ------------------------------------------------------------------------------------------ engine
