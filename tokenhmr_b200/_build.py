@@ -1,8 +1,9 @@
 """Builds libtokenhmr_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU), and next to the test suite
 the probe library tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers
 of every mode, the fused SMPLify-inverse's loss and Adam kernels, and the skeleton overlay's span generator run on the
-host) and the GEMM plan probe tests/libthmr_gemm_probe.so (tests/csrc/gemm_probe.cu: forced epilogue kinds, plan
-queries and the per-tile timeline kernels, which the product does not compile)."""
+host), the GEMM plan probe tests/libthmr_gemm_probe.so (tests/csrc/gemm_probe.cu: forced epilogue kinds, plan
+queries and the per-tile timeline kernels, which the product does not compile) and the regression-head training probe
+tests/libthmr_head_train_probe.so (tests/csrc/head_train_probe.cu: the training kernels of csrc/head_train.cuh)."""
 from __future__ import annotations
 
 import hashlib
@@ -21,6 +22,9 @@ PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_probe.stamp"
 GEMM_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "gemm_probe.cu"
 GEMM_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_gemm_probe.so"
 GEMM_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_gemm_probe.stamp"
+HEAD_PROBE_SRC = PKG_DIR.parent / "tests" / "csrc" / "head_train_probe.cu"
+HEAD_PROBE_PATH = PKG_DIR.parent / "tests" / "libthmr_head_train_probe.so"
+HEAD_PROBE_STAMP = PKG_DIR.parent / "tests" / ".libthmr_head_train_probe.stamp"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -70,11 +74,13 @@ def _compile(src: Path, out: Path, stamp: Path, flags: list, want: str, force: b
 
 
 def build_probe(force: bool = False, verbose: bool = False) -> Path:
-    """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so and tests/csrc/gemm_probe.cu ->
-    tests/libthmr_gemm_probe.so (each a no-op when sources are unchanged)."""
-    if GEMM_PROBE_SRC.exists():
-        _compile(GEMM_PROBE_SRC, GEMM_PROBE_PATH, GEMM_PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, source_hash(probe=True),
-                 force, verbose)
+    """Compile tests/csrc/kernel_probe.cu -> tests/libthmr_probe.so, tests/csrc/gemm_probe.cu ->
+    tests/libthmr_gemm_probe.so and tests/csrc/head_train_probe.cu -> tests/libthmr_head_train_probe.so (each a no-op
+    when sources are unchanged)."""
+    for src, out, stamp in ((GEMM_PROBE_SRC, GEMM_PROBE_PATH, GEMM_PROBE_STAMP),
+                            (HEAD_PROBE_SRC, HEAD_PROBE_PATH, HEAD_PROBE_STAMP)):
+        if src.exists():
+            _compile(src, out, stamp, NVCC_FLAGS + PROBE_FLAGS, source_hash(probe=True), force, verbose)
     return _compile(PROBE_SRC, PROBE_PATH, PROBE_STAMP, NVCC_FLAGS + PROBE_FLAGS, source_hash(probe=True), force,
                     verbose)
 

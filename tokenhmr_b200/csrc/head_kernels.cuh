@@ -88,17 +88,20 @@ __device__ __forceinline__ void rot6d_to_rotmat_one(const float* x, float* R) {
 }
 
 // Backward of rot6d_to_rotmat_one: x the 6D input, g = dL/dR (rows b1, b2, b3) -> gx = dL/dx.  b1 and b2 come from
-// the forward itself; the two norms are recovered as |a1| = a1 . b1 and |u| = a2 . b2 (b2 is orthogonal to b1).  A norm
-// at F.normalize's clamp (1e-12) is a constant, so its projection term drops.
+// the forward itself, and the two norms are taken as the forward takes them, from a1 and u = a2 - (b1 . a2) b1.  (Not
+// as a2 . b2: b2 is orthogonal to b1 only to ~u |a2| / |u|, which dp multiplies again, so for a2 nearly parallel to
+// a1 that recovered |u| loses all its digits and can fall to the clamp.)  A norm at F.normalize's clamp (1e-12) is a
+// constant, so its projection term drops.
 __device__ __forceinline__ void rot6d_to_rotmat_backward_one(const float* x, const float* g, float* gx) {
   float R[9];
   rot6d_to_rotmat_one(x, R);
   const float* b1 = R;
   const float* b2 = R + 3;
   const float* g3 = g + 6;
-  const float r1 = x[0] * b1[0] + x[1] * b1[1] + x[2] * b1[2];
-  const float dp = x[3] * b1[0] + x[4] * b1[1] + x[5] * b1[2];
-  const float r2 = x[3] * b2[0] + x[4] * b2[1] + x[5] * b2[2];
+  const float r1 = sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+  const float dp = b1[0] * x[3] + b1[1] * x[4] + b1[2] * x[5];
+  const float ux = x[3] - dp * b1[0], uy = x[4] - dp * b1[1], uz = x[5] - dp * b1[2];
+  const float r2 = sqrtf(ux * ux + uy * uy + uz * uz);
   const float n1 = fmaxf(r1, 1e-12f), n2 = fmaxf(r2, 1e-12f);
   // b3 = b1 x b2:  dL/db1 += b2 x g3,  dL/db2 += g3 x b1
   float gb1[3] = {g[0] + b2[1] * g3[2] - b2[2] * g3[1], g[1] + b2[2] * g3[0] - b2[0] * g3[2],

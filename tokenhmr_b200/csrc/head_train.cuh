@@ -341,7 +341,9 @@ constexpr long long kSplitFloats = static_cast<long long>(kSplitTarget) * kGBM *
 
 enum HlOrient { kXWt, kDyW, kDytX };
 
-inline void hl_gemm(HlGemm p, HlOrient o, cudaStream_t st) {
+// Split-K count of one GEMM: 1 without a split buffer or when the grid already has kSplitTarget / 2 tiles, else as
+// many splits as fill kSplitTarget CTAs, keeping at least 4 k-blocks per split.
+inline int hl_split_count(const HlGemm& p) {
   const int tn = (p.N + kGBN - 1) / kGBN, tm = (p.M + kGBM - 1) / kGBM;
   const int tiles = tn * tm * p.batch;
   int splits = 1;
@@ -350,6 +352,12 @@ inline void hl_gemm(HlGemm p, HlOrient o, cudaStream_t st) {
     splits = splits < p.K / (4 * kGBK) ? splits : p.K / (4 * kGBK);   // at least 4 k-blocks per split
     if (splits < 1) splits = 1;
   }
+  return splits;
+}
+
+inline void hl_gemm(HlGemm p, HlOrient o, cudaStream_t st) {
+  const int tn = (p.N + kGBN - 1) / kGBN, tm = (p.M + kGBM - 1) / kGBM;
+  const int splits = hl_split_count(p);
   p.splits = splits;
   dim3 grid(tn, tm, p.batch * splits);
   if (o == kXWt) hl_gemm_kernel<true, true><<<grid, 256, 0, st>>>(p);
