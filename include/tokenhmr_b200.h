@@ -331,6 +331,62 @@ int thmr_reg_head_train_forward(const thmr_reg_head_desc* desc);
 int thmr_reg_head_backward(const thmr_reg_head_desc* desc);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training TokenHMR's token head (SMPLTokenDecoderHead, heads/token_head.py:65-128 with IEF_ITERS 1,
+ * TRANSFORMER_INPUT 'zero', JOINT_REP '6d'): the regression head's decoder, then decpose_grot / decshape / deccam /
+ * decpose_hands, the MLP-Mixer token classifier (160 tokens x 64, 4 blocks, 2048 classes) and the frozen tokenizer
+ * decoder (code dim 256, width 512, 21 joints).  fp32 forward that keeps its activations in the workspace, and the
+ * backward to every trainable parameter.
+ *
+ * Two flat fp32 buffers: the trainable parameters (thmr_tok_head_param_info: the reference head's state_dict names
+ * without the init_* buffers, in named_parameters() order) and the frozen tokenizer tensors
+ * (thmr_tok_head_tokenizer_info: tokenizer.decoder.decoder.* and tokenizer.quantizer.codebook), each tensor at a
+ * 64-float aligned offset.  The tokenizer gets no gradient.
+ *
+ * thmr_tok_head_backward reads the activations thmr_tok_head_train_forward left in the same workspace and the
+ * cls_probs it wrote (the workspace holds no second copy), with the same parameters.  It writes every gradient (exact zeros where no upstream gradient reaches), sums over the batch in a
+ * fixed order without atomics, and takes no gradient for the features.  Neither call synchronises the host; both can
+ * be captured in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct thmr_tok_head_desc {
+  int B;                        /* >= 1 */
+  int depth;                    /* 1 .. 64 decoder layers */
+  int heads;                    /* 1 .. 8 (dim_head 64) */
+  int mlp_dim;                  /* 1 .. 16384 */
+  const float* params;          /* flat trainable parameters (thmr_tok_head_param_info layout) */
+  float* grads;                 /* flat gradients, same layout (backward only) */
+  const float* tokenizer;       /* flat frozen tokenizer tensors (thmr_tok_head_tokenizer_info layout) */
+  const float* init_body_pose;  /* [144] */
+  const float* init_betas;      /* [10] */
+  const float* init_cam;        /* [3] */
+  const float* feats;           /* [B,1280,16,12] the backbone's channel-first features */
+  float* pose6d;                /* [B,144] output, may be NULL */
+  float* betas;                 /* [B,10] output */
+  float* cam;                   /* [B,3] output: pred_cam */
+  float* rotmats;               /* [B,24,3,3] output: global_orient, then body_pose */
+  float* cls_probs;             /* [B,160,2048] output: cls_logits_softmax; the backward reads it, unchanged */
+  const float* grad_pose6d;     /* upstream gradients for the backward, each may be NULL (zero): [B,144] */
+  const float* grad_betas;      /* [B,10] */
+  const float* grad_cam;        /* [B,3] */
+  const float* grad_rotmats;    /* [B,24,3,3] */
+  const float* grad_cls_probs;  /* [B,160,2048] */
+  void* workspace;              /* thmr_tok_head_workspace_bytes(B, depth, heads, mlp_dim) bytes, 256-byte aligned */
+  size_t workspace_bytes;
+  void* stream;                 /* cudaStream_t */
+} thmr_tok_head_desc;
+/* Number of trainable parameters and the floats of a flat buffer that holds them. */
+int thmr_tok_head_num_params(int depth, int heads, int mlp_dim, int* count, int64_t* total_floats);
+/* Parameter i: its state_dict name (valid until the next call on this thread), ndim, shape[0..ndim) and its offset in
+ * floats. */
+int thmr_tok_head_param_info(int depth, int heads, int mlp_dim, int i, const char** name, int* ndim, int64_t* shape,
+                             int64_t* offset);
+/* The frozen tokenizer tensors: their count and floats, then tensor i as thmr_tok_head_param_info describes one. */
+int thmr_tok_head_tokenizer_num(int* count, int64_t* total_floats);
+int thmr_tok_head_tokenizer_info(int i, const char** name, int* ndim, int64_t* shape, int64_t* offset);
+size_t thmr_tok_head_workspace_bytes(int B, int depth, int heads, int mlp_dim);
+int thmr_tok_head_train_forward(const thmr_tok_head_desc* desc);
+int thmr_tok_head_backward(const thmr_tok_head_desc* desc);
+
+/* ------------------------------------------------------------------------------------------------
  * Tokenizer encoder + hard quantisation (SURVEY §8 row f4): EncodeTokens
  * [tokenization/models/vanilla_pose_vqvae.py:304-346 -> PoseSPEncoderV1 :42-111, quantize_cnn.py:74-86]
  * ---------------------------------------------------------------------------------------------- */

@@ -55,6 +55,14 @@ class RegHeadDesc(Structure):
                [("workspace_bytes", c_size_t), ("stream", c_void_p)]
 
 
+class TokHeadDesc(Structure):
+    _fields_ = [("B", c_int), ("depth", c_int), ("heads", c_int), ("mlp_dim", c_int)] + \
+               [(n, c_void_p) for n in ("params", "grads", "tokenizer", "init_body_pose", "init_betas", "init_cam",
+                                        "feats", "pose6d", "betas", "cam", "rotmats", "cls_probs", "grad_pose6d",
+                                        "grad_betas", "grad_cam", "grad_rotmats", "grad_cls_probs", "workspace")] + \
+               [("workspace_bytes", c_size_t), ("stream", c_void_p)]
+
+
 class Config(Structure):
     _fields_ = [("image_size", c_int), ("crop_w", c_int), ("patch", c_int), ("patch_pad", c_int),
                 ("vit_dim", c_int), ("vit_depth", c_int), ("vit_heads", c_int), ("vit_mlp_ratio", c_int),
@@ -243,6 +251,15 @@ SIGNATURES = {
     "thmr_reg_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "thmr_reg_head_train_forward": (c_int, [POINTER(RegHeadDesc)]),
     "thmr_reg_head_backward": (c_int, [POINTER(RegHeadDesc)]),
+    "thmr_tok_head_num_params": (c_int, [c_int, c_int, c_int, POINTER(c_int), POINTER(c_int64)]),
+    "thmr_tok_head_param_info": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_char_p), POINTER(c_int),
+                                         POINTER(c_int64), POINTER(c_int64)]),
+    "thmr_tok_head_tokenizer_num": (c_int, [POINTER(c_int), POINTER(c_int64)]),
+    "thmr_tok_head_tokenizer_info": (c_int, [c_int, POINTER(c_char_p), POINTER(c_int), POINTER(c_int64),
+                                             POINTER(c_int64)]),
+    "thmr_tok_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "thmr_tok_head_train_forward": (c_int, [POINTER(TokHeadDesc)]),
+    "thmr_tok_head_backward": (c_int, [POINTER(TokHeadDesc)]),
     "thmr_engine_create": (c_int, [POINTER(Config), POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_create_head": (c_int, [POINTER(Config), c_int, POINTER(Weights), c_void_p, POINTER(c_void_p)]),
     "thmr_engine_destroy": (None, [c_void_p]),

@@ -14,6 +14,9 @@
 // The token-side linears (M = B rows) and every weight gradient (K = B) go through one tiled fp32 kernel
 // (hl_gemm_kernel) in three operand orientations: x W^T, dY W and dY^T X.  Small grids split K and reduce the
 // partials in a fixed order, so a step uses no float atomics, is deterministic, and a graph replay equals eager.
+//
+// The decoder part (rh_layout_decoder, rh_decoder_forward, rh_decoder_backward) is shared with the token head
+// (token_head_train.cuh), which has the same TransformerDecoder under the same transformer.* names.
 #pragma once
 #include <math.h>
 
@@ -51,46 +54,53 @@ enum RhTopSlot { kPos, kTokW, kTokB };
 constexpr int kRhTop = 3, kRhTail = 6;   // pos/token embedding first, then the three read-outs' weight and bias
 
 inline int rh_num_params(int depth) { return kRhTop + depth * kLayerSlots + kRhTail; }
+inline int rh_decoder_params(int depth) { return kRhTop + depth * kLayerSlots; }
 
-// Fills out[0 .. rh_num_params(depth)) in one pass.
-inline void rh_layout(int depth, int heads, int mlp, RhParam* out) {
-  const int n = rh_num_params(depth);
+// One layout entry: name, shape and the next 64-float boundary at or after off.
+inline void rh_set_param(RhParam* q, const char* name, int nd, long long a, long long b, long long c, long long* off) {
+  *q = RhParam{};
+  snprintf(q->name, sizeof(q->name), "%s", name);
+  q->ndim = nd;
+  q->shape[0] = a; q->shape[1] = b; q->shape[2] = c;
+  q->numel = a * (nd > 1 ? b : 1) * (nd > 2 ? c : 1);
+  q->offset = *off;
+  *off += (q->numel + 63) / 64 * 64;
+}
+
+// The decoder's parameters (the transformer.* names both SMPL heads share), out[0 .. rh_decoder_params(depth)).
+// Returns the offset after the last one.
+inline long long rh_layout_decoder(int depth, int heads, int mlp, RhParam* out) {
   const long long E = kRhDim, I = static_cast<long long>(heads) * kRhDimHead, C = kRhCtx, M = mlp;
   long long off = 0;
-  for (int k = 0; k < n; ++k) {
-    RhParam q{};
-    auto set = [&](const char* name, int nd, long long a, long long b, long long c) {
-      snprintf(q.name, sizeof(q.name), "%s", name);
-      q.ndim = nd;
-      q.shape[0] = a; q.shape[1] = b; q.shape[2] = c;
-      q.numel = a * (nd > 1 ? b : 1) * (nd > 2 ? c : 1);
-    };
-    char nm[96];
-    if (k == kPos) set("transformer.pos_embedding", 3, 1, 1, E);
-    else if (k == kTokW) set("transformer.to_token_embedding.weight", 2, E, 1, 0);
-    else if (k == kTokB) set("transformer.to_token_embedding.bias", 1, E, 0, 0);
-    else if (k < kRhTop + depth * kLayerSlots) {
-      const int l = (k - kRhTop) / kLayerSlots, s = (k - kRhTop) % kLayerSlots;
-      static const char* const sfx[kLayerSlots] = {
-          "0.norm.weight", "0.norm.bias", "0.fn.to_qkv.weight", "0.fn.to_out.0.weight", "0.fn.to_out.0.bias",
-          "1.norm.weight", "1.norm.bias", "1.fn.to_kv.weight", "1.fn.to_q.weight", "1.fn.to_out.0.weight",
-          "1.fn.to_out.0.bias", "2.norm.weight", "2.norm.bias", "2.fn.net.0.weight", "2.fn.net.0.bias",
-          "2.fn.net.3.weight", "2.fn.net.3.bias"};
+  rh_set_param(&out[kPos], "transformer.pos_embedding", 3, 1, 1, E, &off);
+  rh_set_param(&out[kTokW], "transformer.to_token_embedding.weight", 2, E, 1, 0, &off);
+  rh_set_param(&out[kTokB], "transformer.to_token_embedding.bias", 1, E, 0, 0, &off);
+  static const char* const sfx[kLayerSlots] = {
+      "0.norm.weight", "0.norm.bias", "0.fn.to_qkv.weight", "0.fn.to_out.0.weight", "0.fn.to_out.0.bias",
+      "1.norm.weight", "1.norm.bias", "1.fn.to_kv.weight", "1.fn.to_q.weight", "1.fn.to_out.0.weight",
+      "1.fn.to_out.0.bias", "2.norm.weight", "2.norm.bias", "2.fn.net.0.weight", "2.fn.net.0.bias",
+      "2.fn.net.3.weight", "2.fn.net.3.bias"};
+  const long long r2[kLayerSlots][2] = {{E, 0}, {E, 0}, {3 * I, E}, {E, I}, {E, 0}, {E, 0}, {E, 0}, {2 * I, C},
+                                        {I, E}, {E, I}, {E, 0}, {E, 0}, {E, 0}, {M, E}, {M, 0}, {E, M}, {E, 0}};
+  char nm[96];
+  for (int l = 0; l < depth; ++l)
+    for (int s = 0; s < kLayerSlots; ++s) {
       snprintf(nm, sizeof(nm), "transformer.transformer.layers.%d.%s", l, sfx[s]);
-      const long long r2[kLayerSlots][2] = {{E, 0}, {E, 0}, {3 * I, E}, {E, I}, {E, 0}, {E, 0}, {E, 0}, {2 * I, C},
-                                            {I, E}, {E, I}, {E, 0}, {E, 0}, {E, 0}, {M, E}, {M, 0}, {E, M}, {E, 0}};
-      set(nm, r2[s][1] ? 2 : 1, r2[s][0], r2[s][1], 0);
-    } else {
-      const int t = k - kRhTop - depth * kLayerSlots;
-      static const char* const names[kRhTail] = {"decpose.weight", "decpose.bias", "decshape.weight",
-                                                 "decshape.bias", "deccam.weight", "deccam.bias"};
-      const long long rows[3] = {kRhPose, kRhBetas, kRhCam};
-      if (t % 2 == 0) set(names[t], 2, rows[t / 2], E, 0);
-      else set(names[t], 1, rows[t / 2], 0, 0);
+      rh_set_param(&out[kRhTop + l * kLayerSlots + s], nm, r2[s][1] ? 2 : 1, r2[s][0], r2[s][1], 0, &off);
     }
-    q.offset = off;
-    off += (q.numel + 63) / 64 * 64;
-    out[k] = q;
+  return off;
+}
+
+// Fills out[0 .. rh_num_params(depth)) in one pass: the decoder, then the three read-outs.
+inline void rh_layout(int depth, int heads, int mlp, RhParam* out) {
+  long long off = rh_layout_decoder(depth, heads, mlp, out);
+  static const char* const names[kRhTail] = {"decpose.weight", "decpose.bias", "decshape.weight", "decshape.bias",
+                                             "deccam.weight", "deccam.bias"};
+  const long long rows[3] = {kRhPose, kRhBetas, kRhCam};
+  for (int t = 0; t < kRhTail; ++t) {
+    RhParam* q = &out[rh_decoder_params(depth) + t];
+    if (t % 2 == 0) rh_set_param(q, names[t], 2, rows[t / 2], kRhDim, 0, &off);
+    else rh_set_param(q, names[t], 1, rows[t / 2], 0, 0, &off);
   }
 }
 
@@ -121,16 +131,22 @@ struct RhPtrs {
   float *pose_w, *pose_b, *betas_w, *betas_b, *cam_w, *cam_b;
 };
 
-inline void rh_pointers(float* base, int depth, int heads, int mlp, RhPtrs* out) {
-  static thread_local RhParam all[kRhMaxParams];
-  rh_layout(depth, heads, mlp, all);
+// The decoder's pointers from a filled layout (rh_layout_decoder's entries come first in both heads' layouts).
+inline void rh_decoder_pointers(float* base, const RhParam* all, int depth, RhPtrs* out) {
   auto at = [&](int i) { return base + all[i].offset; };
   out->pos = at(kPos);
   out->tok_w = at(kTokW);
   out->tok_b = at(kTokB);
   for (int l = 0; l < depth; ++l)
     for (int s = 0; s < kLayerSlots; ++s) out->layer[l].p[s] = at(kRhTop + l * kLayerSlots + s);
-  const int t = kRhTop + depth * kLayerSlots;
+}
+
+inline void rh_pointers(float* base, int depth, int heads, int mlp, RhPtrs* out) {
+  static thread_local RhParam all[kRhMaxParams];
+  rh_layout(depth, heads, mlp, all);
+  rh_decoder_pointers(base, all, depth, out);
+  auto at = [&](int i) { return base + all[i].offset; };
+  const int t = rh_decoder_params(depth);
   out->pose_w = at(t); out->pose_b = at(t + 1);
   out->betas_w = at(t + 2); out->betas_b = at(t + 3);
   out->cam_w = at(t + 4); out->cam_b = at(t + 5);
@@ -610,17 +626,18 @@ inline size_t rh_workspace_bytes(int B, int depth, int H, int mlp) {
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-inline int rh_forward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
-  const int B = d.B, H = d.heads, mlp = d.mlp_dim, E = kRhDim, I = H * kRhDimHead, C = kRhCtx;
+// The decoder's layer loop (both SMPL heads): P's decoder pointers, the channel-first features -> w.tok (B x E), with
+// every layer's activations kept in w.act.
+inline int rh_decoder_forward(const RhPtrs& P, const float* feats, int B, int depth, int H, int mlp, RhWs& w,
+                              cudaStream_t st) {
+  const int E = kRhDim, I = H * kRhDimHead, C = kRhCtx;
   const float scale = 1.f / sqrtf(static_cast<float>(kRhDimHead));
-  RhPtrs P;
-  rh_pointers(const_cast<float*>(d.params), d.depth, H, mlp, &P);
   THMR_TRY(rh_configure());
   rh_token0_kernel<<<(B * E + 255) / 256, 256, 0, st>>>(P.tok_b, P.pos, w.act[0].x0, B);
-  for (int l = 0; l < d.depth; ++l) {
+  for (int l = 0; l < depth; ++l) {
     RhLayerAct& a = w.act[l];
-    float** L = P.layer[l].p;
-    float* xout = l + 1 < d.depth ? w.act[l + 1].x0 : w.tok;
+    float* const* L = P.layer[l].p;
+    float* xout = l + 1 < depth ? w.act[l + 1].x0 : w.tok;
     // self-attention over one key: x1 = x0 + to_out(W_v LN0(x0))
     rh_ln_fwd_kernel<<<B, 256, 0, st>>>(a.x0, L[kL0g], L[kL0b], a.y0, a.mean, a.rstd);
     hl_linear(a.y0, E, L[kQkv] + static_cast<size_t>(2) * I * E, nullptr, a.v, I, B, I, E, false, nullptr, w.split, st);
@@ -637,7 +654,7 @@ inline int rh_forward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
       p.C = w.kq; p.ldc = static_cast<long long>(H) * C; p.sCz = C;
       hl_gemm(p, kDyW, st);
     }
-    rh_attn_chunk_kernel<false><<<dim3(kRhChunks, B), 256, kRhAttSmem, st>>>(d.feats, w.kq, H, scale, a.s, nullptr,
+    rh_attn_chunk_kernel<false><<<dim3(kRhChunks, B), 256, kRhAttSmem, st>>>(feats, w.kq, H, scale, a.s, nullptr,
                                                                             nullptr, nullptr, w.stat, w.part);
     rh_attn_combine_kernel<<<B * H, 256, 0, st>>>(w.part, w.stat, H, a.c, a.lse);
     {
@@ -656,6 +673,14 @@ inline int rh_forward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
     THMR_CUDA(cudaMemcpyAsync(xout, a.x2, sizeof(float) * B * E, cudaMemcpyDeviceToDevice, st));
     hl_linear(a.h, mlp, L[kF2w], L[kF2b], xout, E, B, E, mlp, true, nullptr, w.split, st);
   }
+  return THMR_OK;
+}
+
+inline int rh_forward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
+  const int B = d.B, E = kRhDim;
+  RhPtrs P;
+  rh_pointers(const_cast<float*>(d.params), d.depth, d.heads, d.mlp_dim, &P);
+  THMR_TRY(rh_decoder_forward(P, d.feats, B, d.depth, d.heads, d.mlp_dim, w, st));
   // read-outs (smpl_head.py:82-84) into [pose | betas | cam], then + init_* and rot6d_to_rotmat (:89-99)
   hl_linear(w.tok, E, P.pose_w, P.pose_b, w.read, kRhReadLd, B, kRhPose, E, false, nullptr, w.split, st);
   hl_linear(w.tok, E, P.betas_w, P.betas_b, w.read + kRhPose, kRhReadLd, B, kRhBetas, E, false, nullptr, w.split, st);
@@ -671,31 +696,18 @@ inline int rh_forward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-inline int rh_backward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
-  const int B = d.B, H = d.heads, mlp = d.mlp_dim, E = kRhDim, I = H * kRhDimHead, C = kRhCtx;
+// The decoder's layer loop backward (both SMPL heads): from d tok in w.dx to the gradient of every decoder parameter
+// (G's decoder pointers), reading the activations rh_decoder_forward kept.
+inline int rh_decoder_backward(const RhPtrs& P, const RhPtrs& G, const float* feats, int B, int depth, int H, int mlp,
+                               RhWs& w, cudaStream_t st) {
+  const int E = kRhDim, I = H * kRhDimHead, C = kRhCtx;
   const float scale = 1.f / sqrtf(static_cast<float>(kRhDimHead));
-  RhPtrs P, G;
-  rh_pointers(const_cast<float*>(d.params), d.depth, H, mlp, &P);
-  rh_pointers(d.grads, d.depth, H, mlp, &G);
   THMR_TRY(rh_configure());
   const unsigned colE = (E + 127) / 128;
-  // read-outs
-  rh_readout_bwd_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(w.pose6d, d.grad_rotmats, d.grad_pose6d, d.grad_betas,
-                                                              d.grad_cam, w.dread, B);
-  const int rows[3] = {kRhPose, kRhBetas, kRhCam}, col[3] = {0, kRhPose, kRhPose + kRhBetas};
-  float* const rw[3] = {P.pose_w, P.betas_w, P.cam_w};
-  float* const gw[3] = {G.pose_w, G.betas_w, G.cam_w};
-  float* const gb[3] = {G.pose_b, G.betas_b, G.cam_b};
-  for (int r = 0; r < 3; ++r) {
-    hl_linear_dw(w.dread + col[r], kRhReadLd, w.tok, E, gw[r], B, rows[r], E, 1.f, st);
-    rh_colsum_kernel<<<1, 256, 0, st>>>(w.dread + col[r], kRhReadLd, B, rows[r], gb[r], nullptr, nullptr, nullptr,
-                                        nullptr, nullptr);
-    hl_linear_dx(w.dread + col[r], kRhReadLd, rw[r], w.dx, E, B, rows[r], E, r > 0, nullptr, w.split, st);
-  }
-  for (int l = d.depth - 1; l >= 0; --l) {
+  for (int l = depth - 1; l >= 0; --l) {
     RhLayerAct& a = w.act[l];
-    float** L = P.layer[l].p;
-    float** Lg = G.layer[l].p;
+    float* const* L = P.layer[l].p;
+    float* const* Lg = G.layer[l].p;
     // feed-forward
     rh_colsum_kernel<<<colE, 128, 0, st>>>(w.dx, E, B, E, Lg[kF2b], nullptr, nullptr, nullptr, nullptr, nullptr);
     hl_linear_dw(w.dx, E, a.h, mlp, Lg[kF2w], B, E, mlp, 1.f, st);
@@ -727,7 +739,7 @@ inline int rh_backward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
       p.C = Lg[kKv] + static_cast<size_t>(I) * C; p.ldc = C; p.sCz = static_cast<long long>(kRhDimHead) * C;
       hl_gemm(p, kDytX, st);
     }
-    rh_attn_chunk_kernel<true><<<dim3(kRhChunks, B), 256, kRhAttSmem, st>>>(d.feats, w.dtil, H, scale, a.s, a.lse,
+    rh_attn_chunk_kernel<true><<<dim3(kRhChunks, B), 256, kRhAttSmem, st>>>(feats, w.dtil, H, scale, a.s, a.lse,
                                                                            w.dI, a.o, nullptr, w.part);
     rh_attn_combine_kernel<<<B * H, 256, 0, st>>>(w.part, nullptr, H, w.uatt, nullptr);
     {
@@ -766,6 +778,28 @@ inline int rh_backward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
   // multiplies a zero input
   rh_colsum_kernel<<<colE, 128, 0, st>>>(w.dx, E, B, E, G.tok_b, G.pos, nullptr, nullptr, nullptr, nullptr);
   THMR_CUDA(cudaMemsetAsync(G.tok_w, 0, sizeof(float) * E, st));
+  return THMR_OK;
+}
+
+inline int rh_backward(const thmr_reg_head_desc& d, RhWs& w, cudaStream_t st) {
+  const int B = d.B, H = d.heads, mlp = d.mlp_dim, E = kRhDim;
+  RhPtrs P, G;
+  rh_pointers(const_cast<float*>(d.params), d.depth, H, mlp, &P);
+  rh_pointers(d.grads, d.depth, H, mlp, &G);
+  // read-outs
+  rh_readout_bwd_kernel<<<(B * 24 + 127) / 128, 128, 0, st>>>(w.pose6d, d.grad_rotmats, d.grad_pose6d, d.grad_betas,
+                                                              d.grad_cam, w.dread, B);
+  const int rows[3] = {kRhPose, kRhBetas, kRhCam}, col[3] = {0, kRhPose, kRhPose + kRhBetas};
+  float* const rw[3] = {P.pose_w, P.betas_w, P.cam_w};
+  float* const gw[3] = {G.pose_w, G.betas_w, G.cam_w};
+  float* const gb[3] = {G.pose_b, G.betas_b, G.cam_b};
+  for (int r = 0; r < 3; ++r) {
+    hl_linear_dw(w.dread + col[r], kRhReadLd, w.tok, E, gw[r], B, rows[r], E, 1.f, st);
+    rh_colsum_kernel<<<1, 256, 0, st>>>(w.dread + col[r], kRhReadLd, B, rows[r], gb[r], nullptr, nullptr, nullptr,
+                                        nullptr, nullptr);
+    hl_linear_dx(w.dread + col[r], kRhReadLd, rw[r], w.dx, E, B, rows[r], E, r > 0, nullptr, w.split, st);
+  }
+  THMR_TRY(rh_decoder_backward(P, G, d.feats, B, d.depth, H, mlp, w, st));
   THMR_CUDA(cudaGetLastError());
   return THMR_OK;
 }

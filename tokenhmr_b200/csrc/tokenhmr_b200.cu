@@ -9,6 +9,7 @@
 #include "engine_strict.cuh"
 #include "eval_kernels.cuh"
 #include "head_train.cuh"
+#include "token_head_train.cuh"
 #include "keypoints.cuh"
 #include "losses.cuh"
 #include "preproc.cuh"
@@ -978,6 +979,96 @@ int thmr_reg_head_backward(const thmr_reg_head_desc* d) {
   static thread_local RhWs ws;
   THMR_TRY(reg_head_check(d, true, &ws));
   return rh_backward(*d, ws, static_cast<cudaStream_t>(d->stream));
+}
+
+// ------------------------------------------------------------------------------------------ token-head training
+static int head_info_out(const RhParam& p, const char** name, int* ndim, int64_t* shape, int64_t* offset) {
+  *name = p.name;
+  *ndim = p.ndim;
+  for (int k = 0; k < p.ndim; ++k) shape[k] = p.shape[k];
+  *offset = p.offset;
+  return THMR_OK;
+}
+
+int thmr_tok_head_num_params(int depth, int heads, int mlp_dim, int* count, int64_t* total_floats) {
+  THMR_CHECK(count && total_floats, "tok_head_num_params: null argument");
+  THMR_CHECK(reg_head_dims_ok(depth, heads, mlp_dim),
+             "tok_head: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)",
+             depth, heads, mlp_dim, kRhMaxHeads);
+  *count = tk_num_params(depth);
+  *total_floats = tk_param_floats(depth, heads, mlp_dim);
+  return THMR_OK;
+}
+
+int thmr_tok_head_param_info(int depth, int heads, int mlp_dim, int i, const char** name, int* ndim, int64_t* shape,
+                             int64_t* offset) {
+  static thread_local RhParam p;
+  THMR_CHECK(name && ndim && shape && offset, "tok_head_param_info: null argument");
+  THMR_CHECK(reg_head_dims_ok(depth, heads, mlp_dim),
+             "tok_head: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)",
+             depth, heads, mlp_dim, kRhMaxHeads);
+  THMR_CHECK(tk_param(depth, heads, mlp_dim, i, &p), "tok_head_param_info: index %d outside [0, %d)", i,
+             tk_num_params(depth));
+  return head_info_out(p, name, ndim, shape, offset);
+}
+
+int thmr_tok_head_tokenizer_num(int* count, int64_t* total_floats) {
+  THMR_CHECK(count && total_floats, "tok_head_tokenizer_num: null argument");
+  *count = kTkTokTensors;
+  *total_floats = tk_tokenizer_floats();
+  return THMR_OK;
+}
+
+int thmr_tok_head_tokenizer_info(int i, const char** name, int* ndim, int64_t* shape, int64_t* offset) {
+  static thread_local RhParam p;
+  THMR_CHECK(name && ndim && shape && offset, "tok_head_tokenizer_info: null argument");
+  THMR_CHECK(tk_tokenizer_param(i, &p), "tok_head_tokenizer_info: index %d outside [0, %d)", i, kTkTokTensors);
+  return head_info_out(p, name, ndim, shape, offset);
+}
+
+size_t thmr_tok_head_workspace_bytes(int B, int depth, int heads, int mlp_dim) {
+  if (B < 1 || !reg_head_dims_ok(depth, heads, mlp_dim)) return 0;
+  return tk_workspace_bytes(B, depth, heads, mlp_dim);
+}
+
+static int tok_head_check(const thmr_tok_head_desc* d, bool backward, TkWs* ws) {
+  const char* what = backward ? "tok_head_backward" : "tok_head_train_forward";
+  THMR_CHECK(d, "%s: null descriptor", what);
+  THMR_CHECK(d->B >= 1, "%s: B=%d (must be >= 1)", what, d->B);
+  THMR_CHECK(reg_head_dims_ok(d->depth, d->heads, d->mlp_dim),
+             "%s: unsupported dims depth=%d heads=%d mlp_dim=%d (depth 1..64, heads 1..%d, mlp_dim 1..16384)", what,
+             d->depth, d->heads, d->mlp_dim, kRhMaxHeads);
+  THMR_CHECK(d->params && d->tokenizer && d->feats && d->init_body_pose && d->init_betas && d->init_cam,
+             "%s: null input pointer", what);
+  THMR_CHECK(d->workspace, "%s: null workspace", what);
+  const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  THMR_CHECK((reinterpret_cast<uintptr_t>(d->workspace) & 255) == 0 && a16(d->params) && a16(d->tokenizer) &&
+                 (!d->grads || a16(d->grads)) && (!d->cls_probs || a16(d->cls_probs)) &&
+                 (!d->grad_cls_probs || a16(d->grad_cls_probs)),
+             "%s: workspace must be 256-byte and params / tokenizer / grads 16-byte aligned", what);
+  const size_t need = tk_workspace_bytes(d->B, d->depth, d->heads, d->mlp_dim);
+  THMR_CHECK(d->workspace_bytes >= need, "%s: workspace too small: %zu bytes, need %zu", what, d->workspace_bytes,
+             need);
+  if (backward) {
+    THMR_CHECK(d->grads, "%s: null gradient buffer", what);
+    THMR_CHECK(d->cls_probs, "%s: null cls_probs (the forward's cls_logits_softmax, which the backward reads)", what);
+  } else {
+    THMR_CHECK(d->betas && d->cam && d->rotmats && d->cls_probs, "%s: null output pointer", what);
+  }
+  tk_carve(static_cast<float*>(d->workspace), d->B, d->depth, d->heads, d->mlp_dim, ws);
+  return THMR_OK;
+}
+
+int thmr_tok_head_train_forward(const thmr_tok_head_desc* d) {
+  static thread_local TkWs ws;
+  THMR_TRY(tok_head_check(d, false, &ws));
+  return tk_forward(*d, ws, static_cast<cudaStream_t>(d->stream));
+}
+
+int thmr_tok_head_backward(const thmr_tok_head_desc* d) {
+  static thread_local TkWs ws;
+  THMR_TRY(tok_head_check(d, true, &ws));
+  return tk_backward(*d, ws, static_cast<cudaStream_t>(d->stream));
 }
 
 // ------------------------------------------------------------------------------------------ engine
