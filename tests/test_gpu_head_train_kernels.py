@@ -12,7 +12,6 @@ NaN, so an unwritten element fails, and pitch padding must still be NaN afterwar
 two results must be identical.  Each bound family also shows it has teeth: it rejects an fp64 reference with one term
 taken out."""
 import dataclasses
-import zlib
 
 import pytest
 import torch
@@ -20,6 +19,7 @@ import torch.nn.functional as F
 
 import head_train_probe as hp
 import probe
+from head_train_probe import Site, _linear, _linear_dw, _linear_dx, _nan, _rejects, _twice, gamma
 from oracle import regression_oracle as R
 from oracle import tokenhmr_oracle as O
 from probe import U32, assert_within
@@ -40,107 +40,9 @@ def _flags(cuda_dev, built_lib):
     assert built_lib.thmr_check_device_flags() == 0, built_lib.thmr_last_error()
 
 
-def _nan(*shape):
-    return torch.full(shape, float("nan"), device="cuda")
-
-
-def gamma(n: int) -> float:
-    """gamma_n = n u / (1 - n u): the relative error bound of n chained fp32 roundings."""
-    return n * U32 / (1 - n * U32)
-
-
-def _rejects(got, ref, bound) -> bool:
-    """True when some element of got lies outside bound of the (perturbed) reference."""
-    err = (got.double() - ref.double()).abs()
-    return bool((~(err <= torch.as_tensor(bound, device=err.device).double())).any())
-
-
-def _twice(run):
-    """Runs a launch twice; the two results must be bit-identical (no atomics, fixed reduction order)."""
-    a = run()
-    b = run()
-    for x, y in zip(a, b):
-        assert torch.equal(x.nan_to_num(1234.5), y.nan_to_num(1234.5)) and torch.equal(x.isnan(), y.isnan())
-    return a
-
-
 # ------------------------------------------------------------------------------------------------ hl_gemm
-# C[z] = epilogue(alpha * sum_k A(m,k) B(k,n)).  Each output is a serial fmaf chain over its split's k range (at most
-# kper = ceil(K / splits) terms), then, when split, the reduce kernel's `splits` additions in split order, so every
-# product passes through at most kper + splits roundings: |acc - S| <= gamma_(kper+splits) sum_k |a||b| (= Tab).
-# Then alpha (a power of two here: exact), + bias (1 rounding), * gelu'(dgelu) (1 rounding), + C0 (1 rounding): with
-# G the fp64 gelu' (1 without dgelu) and eps_G the error of the fp32 gelu' itself,
-#   |C - C64| <= gamma_(kper+splits+4) |G| (|alpha| Tab + |bias|) + eps_G (|alpha| Tab + |bias|) + u |C0|.
-# gelu'(x) = 0.5 (1 + erff(x / sqrt 2)) + x phi(x) with expf: erff's 2 ulp and the argument's rounding (erf' <= 1.13)
-# give u (2 + 0.8 |x|) on the first half; expf's 2 ulp, the rounding of -x^2/2 (relative u x^2 / 2 on the result) and
-# three products on |x phi(x)| <= 0.25; the final sum u |G| <= 1.13 u:  eps_G = u (8 + |x| + x^2 |x| phi(x)).
-# gelu_out = gelu(C) in fp32: |gelu'| <= 1.13 carries C's error; erff's 2 ulp and the argument's rounding on
-# 0.5 |x| (1 + erf), the two products and (1 + erf)'s rounding add at most 4 u (|x| + 1).
-FLOOR = 1e-30
-
-
-def _gelu_grad64(x):
-    return 0.5 * (1 + torch.erf(x / 2 ** 0.5)) + x * torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
-
-
-def _eps_gelu_grad(x):
-    phi = torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
-    return U32 * (8 + x.abs() + x * x * x.abs() * phi)
-
-
-def _view(buf, off, strides, size):
-    return torch.as_strided(buf, size, strides, off)
-
-
-@dataclasses.dataclass
-class Site:
-    """One hl_gemm call: orientation, shape, operand strides (batch, row, col) and offsets into flat buffers, epilogue,
-    and the split count the planner must choose."""
-    name: str
-    orient: str
-    M: int
-    N: int
-    K: int
-    batch: int
-    sA: tuple           # (sAz, sAm, sAk)
-    sB: tuple           # (sBz, sBk, sBn)
-    sC: tuple           # (sCz, ldc, 1)
-    splits: int
-    a_off: int = 0
-    b_off: int = 0
-    c_off: int = 0
-    c_extent: int = 0   # size of the output buffer (0: just what the view covers)
-    alpha: float = 1.0
-    bias: bool = False
-    accumulate: bool = False
-    dgelu: bool = False
-    gelu_out: bool = False
-    partial: bool = True
-
-
-def _extent(off, strides, size):
-    return off + sum((n - 1) * s for n, s in zip(size, strides)) + 1
-
-
-def _linear(name, B, N, K, splits, ldx=None, ldy=None, y_off=0, y_extent=0, **kw):
-    """hl_linear: y (B x N, ld ldy) [+]= x (B x K, ld ldx) W^T + bias."""
-    ldx, ldy = ldx or K, ldy or N
-    return Site(name, "xwt", B, N, K, 1, (0, ldx, 1), (0, 1, K), (0, ldy, 1), splits, c_off=y_off,
-                c_extent=y_extent, **kw)
-
-
-def _linear_dx(name, B, N, K, splits, ldy=None, y_off=0, **kw):
-    """hl_linear_dx: dx (B x K) [+]= dy (B x N, ld ldy) W, W: N x K."""
-    ldy = ldy or N
-    return Site(name, "dyw", B, K, N, 1, (0, ldy, 1), (0, K, 1), (0, K, 1), splits, a_off=y_off, **kw)
-
-
-def _linear_dw(name, B, N, K, ldy=None, y_off=0, ldx=None):
-    """hl_linear_dw: dW (N x K) = dy^T (B x N, ld ldy) x (B x K, ld ldx); no split buffer."""
-    ldy, ldx = ldy or N, ldx or K
-    return Site(name, "dytx", N, K, B, 1, (0, 1, ldy), (0, ldx, 1), (0, K, 1), 1, a_off=y_off, partial=False)
-
-
+# The call-site machinery (Site, its fp64 reference and the derivation of its bound) is in head_train_probe.py,
+# shared with the token head's call sites in tests/test_gpu_token_head_train_kernels.py.
 def _per_head(kind, H, B, splits):
     """The six batched per-head call sites of rh_forward / rh_backward, with their real strides: q, dO, o, dq are
     B x I (I = 64 H); kq, d~, c, u are B x H x 1280; W_k, W_v are the two halves of to_kv (2I x 1280)."""
@@ -217,67 +119,6 @@ def test_site_table_covers_every_planner_branch():
     assert {s.batch for s in SITES} >= {1, 3, 8}
 
 
-def _operands(site, integer: bool, g):
-    """Flat fp32 buffers of A, B, bias, dgelu and C0 (C0: the accumulate input, NaN outside the view)."""
-    Asz, Bsz, Csz = (site.batch, site.M, site.K), (site.batch, site.K, site.N), (site.batch, site.M, site.N)
-    draw = ((lambda n: torch.randint(-4, 5, (n,), device="cuda", generator=g).float()) if integer else
-            (lambda n: torch.randn(n, device="cuda", generator=g)))
-    A = draw(_extent(site.a_off, site.sA, Asz))
-    Bm = draw(_extent(site.b_off, site.sB, Bsz))
-    c_ext = max(site.c_extent, _extent(site.c_off, site.sC, Csz))
-    C0 = torch.full((c_ext,), float("nan"), device="cuda")
-    if site.accumulate:
-        _view(C0, site.c_off, site.sC, Csz).copy_(draw(site.batch * site.M * site.N).view(Csz))
-    bias = (draw(site.N) * (2 if integer else 1)) if site.bias else None
-    dg = None
-    if site.dgelu and not integer:
-        dg = torch.zeros(c_ext, device="cuda")
-        _view(dg, site.c_off, site.sC, Csz).copy_(2 * torch.randn(Csz, device="cuda", generator=g))
-    return A, Bm, bias, dg, C0
-
-
-def _run_site(site, A, Bm, bias, dg, C0, split):
-    Csz = (site.batch, site.M, site.N)
-    out, gout = C0.clone(), (torch.full_like(C0, float("nan")) if site.gelu_out else None)
-    d = hp.HlGemm(A=A.data_ptr() + 4 * site.a_off, sAz=site.sA[0], sAm=site.sA[1], sAk=site.sA[2],
-                     Bm=Bm.data_ptr() + 4 * site.b_off, sBz=site.sB[0], sBk=site.sB[1], sBn=site.sB[2],
-                     C=out.data_ptr() + 4 * site.c_off, sCz=site.sC[0], ldc=site.sC[1],
-                     M=site.M, N=site.N, K=site.K, batch=site.batch, alpha=site.alpha,
-                     bias=probe.ptr(bias), dgelu=None if dg is None else dg.data_ptr() + 4 * site.c_off,
-                     gelu_out=None if gout is None else gout.data_ptr() + 4 * site.c_off,
-                     accumulate=int(site.accumulate), partial=probe.ptr(split) if site.partial else None, splits=-7)
-    n = hp.hl_gemm(d, site.orient)
-    torch.cuda.synchronize()
-    assert n == site.splits, f"{site.name}: {n} splits, the table says {site.splits}"
-    return (out, gout) if gout is not None else (out,)
-
-
-def _reference(site, A, Bm, bias, dg, C0, kmask=None):
-    """fp64 epilogue(alpha * A B) over the k set kmask (all k by default), and the bound's ingredients."""
-    Asz, Bsz, Csz = (site.batch, site.M, site.K), (site.batch, site.K, site.N), (site.batch, site.M, site.N)
-    a = _view(A.double(), site.a_off, site.sA, Asz)
-    b = _view(Bm.double(), site.b_off, site.sB, Bsz)
-    am = a if kmask is None else a * kmask.view(1, 1, -1)
-    S = site.alpha * (am @ b)
-    Tab = abs(site.alpha) * (a.abs() @ b.abs())
-    v = S + (bias.double() if bias is not None else 0)
-    mag = Tab + (bias.double().abs() if bias is not None else 0)
-    G, epsG = 1.0, 0.0
-    if dg is not None:
-        x = _view(dg.double(), site.c_off, site.sC, Csz)
-        G, epsG = _gelu_grad64(x), _eps_gelu_grad(x)
-        v = v * G
-    c0 = _view(C0.double(), site.c_off, site.sC, Csz) if site.accumulate else 0
-    v = v + c0
-    return v, mag, G, epsG, c0
-
-
-def _covered(site, n):
-    m = torch.zeros(n, dtype=torch.bool, device="cuda")
-    _view(m, site.c_off, site.sC, (site.batch, site.M, site.N)).fill_(True)
-    return m
-
-
 @pytest.fixture(scope="module")
 def split_buf(cuda_dev):
     n = hp.lib().head_probe_hl_split_floats()
@@ -287,53 +128,12 @@ def split_buf(cuda_dev):
 
 @pytest.mark.parametrize("site", SITES, ids=[s.name for s in SITES])
 def test_hl_gemm_integer_exact(site, split_buf):
-    """Integer operands in [-4, 4], an integer bias and C0, alpha a power of two: every partial sum is an integer below
-    2^24 (|sum| <= 16 K), so the result equals fp64 exactly; a dropped, doubled or misindexed term fails.  dgelu rows
-    run without dgelu here."""
-    g = torch.Generator(device="cuda").manual_seed(zlib.crc32(site.name.encode()))
-    A, Bm, bias, dg, C0 = _operands(site, True, g)
-    outs = _twice(lambda: _run_site(site, A, Bm, bias, None, C0, split_buf))
-    Csz = (site.batch, site.M, site.N)
-    ref, *_ = _reference(site, A, Bm, bias, None, C0)
-    got = _view(outs[0], site.c_off, site.sC, Csz)
-    assert torch.equal(got.double(), ref), f"{site.name}: {int((got.double() != ref).sum())} elements differ"
-    cov = _covered(site, outs[0].numel())
-    assert outs[0][~cov].isnan().all(), "wrote outside the output view"
-    if site.gelu_out:       # gelu of an exact value: only gelu's own error (the bound below with C's error 0)
-        x = ref
-        assert_within(f"hl_gemm gelu_out (integer) {site.name}", _view(outs[1], site.c_off, site.sC, Csz),
-                      probe.gelu64(x), 4 * U32 * (x.abs() + 1) + FLOOR)
-        assert outs[1][~cov].isnan().all()
+    hp.check_site_integer_exact(site, split_buf)
 
 
 @pytest.mark.parametrize("site", SITES, ids=[s.name for s in SITES])
 def test_hl_gemm_random_within_bound(site, split_buf):
-    g = torch.Generator(device="cuda").manual_seed(7 + zlib.crc32(site.name.encode()))
-    A, Bm, bias, dg, C0 = _operands(site, False, g)
-    outs = _twice(lambda: _run_site(site, A, Bm, bias, dg, C0, split_buf))
-    Csz = (site.batch, site.M, site.N)
-    kper = (site.K + site.splits - 1) // site.splits
-    n = kper + (site.splits if site.splits > 1 else 0)
-    ref, mag, G, epsG, c0 = _reference(site, A, Bm, bias, dg, C0)
-    absG = G.abs() if torch.is_tensor(G) else G
-    c0a = c0.abs() if torch.is_tensor(c0) else 0
-    bound = gamma(n + 4) * absG * mag + epsG * mag + U32 * c0a + FLOOR
-    got = _view(outs[0], site.c_off, site.sC, Csz)
-    assert_within(f"hl_gemm {site.name}", got, ref, bound)
-    cov = _covered(site, outs[0].numel())
-    assert outs[0][~cov].isnan().all(), "wrote outside the output view"
-    if site.gelu_out:
-        assert_within(f"hl_gemm gelu_out {site.name}", _view(outs[1], site.c_off, site.sC, Csz), probe.gelu64(ref),
-                      1.13 * bound + 4 * U32 * (ref.abs() + 1))
-        assert outs[1][~cov].isnan().all()
-    # teeth: the same bound rejects the reference without one k-term, and without one split's partial
-    mask = torch.ones(site.K, dtype=torch.float64, device="cuda")
-    mask[site.K // 2] = 0
-    assert _rejects(got, _reference(site, A, Bm, bias, dg, C0, mask)[0], bound), "bound accepts a dropped k-term"
-    if site.splits > 1:
-        mask = torch.ones(site.K, dtype=torch.float64, device="cuda")
-        mask[kper:min(site.K, 2 * kper)] = 0
-        assert _rejects(got, _reference(site, A, Bm, bias, dg, C0, mask)[0], bound), "bound accepts a dropped split"
+    hp.check_site_within_bound(site, split_buf)
 
 
 # ------------------------------------------------------------------------------------------------ cross-attention

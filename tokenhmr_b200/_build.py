@@ -2,8 +2,9 @@
 the probe library tests/libthmr_probe.so (tests/csrc/kernel_probe.cu: test-only wrappers around the internal launchers
 of every mode, the fused SMPLify-inverse's loss and Adam kernels, and the skeleton overlay's span generator run on the
 host), the GEMM plan probe tests/libthmr_gemm_probe.so (tests/csrc/gemm_probe.cu: forced epilogue kinds, plan
-queries and the per-tile timeline kernels, which the product does not compile) and the regression-head training probe
-tests/libthmr_head_train_probe.so (tests/csrc/head_train_probe.cu: the training kernels of csrc/head_train.cuh)."""
+queries and the per-tile timeline kernels, which the product does not compile) and the head-training probe
+tests/libthmr_head_train_probe.so (tests/csrc/head_train_probe.cu: the training kernels of csrc/head_train.cuh and
+csrc/token_head_train.cuh)."""
 from __future__ import annotations
 
 import hashlib
